@@ -16,9 +16,8 @@ horizon 32 (SURVEY.md section 8d).  Prints ONE JSON line (rank 0):
                C ABI on resident inputs (pre-scaled joint_act, random cotangents), CUDA events, max over ranks.  It explains
                ``e2e``; it is not the claim.
 * ``roofline`` dominant kernel (the adjoint launch): ``frac`` = SURVEY.md section 8d's algorithmic bytes (state-only tape:
-               2 200 B per Ant env-step adjoint) x environments / measured launch time / measured HBM peak.  ``design_frac`` =
-               the same with the bytes this design really moves (tape rows incl. the forward intermediates + H^-1 blocks);
-               ``fp32`` = executed fp32 FLOP against the CUDA-core peak: the path is issue / latency bound, not HBM bound.
+               2 200 B per Ant env-step adjoint) x environments / measured launch time / HBM peak.  ``design_frac`` =
+               the same with the bytes this design really moves (tape rows incl. the forward intermediates + H^-1 blocks).
 * ``configs``  the other named configs of BASELINE.json, each with value / e2e / kernel_ms / section-8d roofline:
                ``humanoid8192`` (C2, fp32 tape) and ``humanoid8192_bf16_tape`` (C2 as named: "bf16 states" -- the tape stores the
                link velocities, bias accelerations and wrenches of every row as bf16; arithmetic and the state stay fp32),
@@ -26,9 +25,11 @@ horizon 32 (SURVEY.md section 8d).  Prints ONE JSON line (rank 0):
                ``c4``: Ant at 8192 envs per GPU with the policy-gradient all-reduce (C4).
 * ``cpu_baseline`` / ``gpu_baseline``  the UNMODIFIED reference through its own public API (``oracle/ref_gpu_arm.py`` on the
                install under ``baseline/_ref``): its CPU path on one host core, and its CUDA codegen path (rebuilt for
-               sm_100, one flag edit) on this GPU at the headline config -- the only pre-existing GPU implementation.
+               sm_90, one flag edit) on this GPU at the headline config -- the only pre-existing GPU implementation.
 * ``--impl reference`` times the reference CPU path on all host cores (one single-threaded process per core, wall-clocked);
   ``--impl reference-cuda`` the reference CUDA path; both print the same line shape with ``"impl": "reference"``.
+``--steps K`` = timed rollouts of every timed loop.  ``--dump-outputs DIR``: the kernel path's and the e2e path's results of
+the headline's last timed rollout as DIR/<name>.npy (seeded inputs: two builds compare output for output).
 """
 import argparse
 import json
@@ -73,7 +74,7 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0}, "fallback: H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -160,14 +161,14 @@ def cpu_reference_baseline(env_name):
 
 
 def gpu_reference_baseline(env_name, num_envs, horizon, rollouts=2):
-    """The reference's own CUDA codegen path (sm_100 rebuild) on this GPU at the same config: the GPU-vs-GPU bar."""
+    """The reference's own CUDA codegen path (sm_90 rebuild) on this GPU at the same config: the GPU-vs-GPU bar."""
     r = _run_ref_arm(_ref_arm_cmd(env_name, num_envs, horizon, rollouts, 1, "cuda:0"), 900)
     if "unavailable" in r:
         return {"value": None, "unit": "env-steps/s", "kind": "reference-cuda", "unavailable": r["unavailable"]}
     return {"value": r["env_steps_per_s"], "unit": "env-steps/s", "kind": "reference-cuda", "api": r["api"],
             "config": "%s num_envs=%d horizon=%d, %d timed rollouts" % (env_name, num_envs, horizon, rollouts),
             "forward_s": r["forward_s"], "backward_s": r["backward_s"], "finite": r["finite"], "peak_mem_gb": r["peak_mem_gb"],
-            "note": "reference CUDA codegen (dflex/dflex/adjoint.py:1247-1262) with the one flag edit compute_35 -> compute_100 "
+            "note": "reference CUDA codegen (dflex/dflex/adjoint.py:1247-1262) with the one flag edit compute_35 -> compute_90 "
                     "(adjoint.py:1861), driven through the reference's stock envs.%s.step; host-timed with synchronize "
                     "(Python launch overhead is part of the reference path)" % env_name}
 
@@ -238,7 +239,7 @@ def run_reference_cuda(args):
     line = {"impl": "reference", "metric": METRIC, "value": g["value"], "unit": "env-steps/s", "n_gpus": 1,
             "steps": max(1, args.steps), "warmup": 1, "ms_per_step": 1e3 * secs / max(1, args.steps), "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-            "config": {"workload": "%s num_envs=%d horizon=%d on the reference's CUDA codegen path (sm_100 rebuild)" % (args.env, args.num_envs, T)},
+            "config": {"workload": "%s num_envs=%d horizon=%d on the reference's CUDA codegen path (sm_90 rebuild)" % (args.env, args.num_envs, T)},
             "gpu_baseline": g,
             "e2e": {"value": g["value"], "unit": "env-steps/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line))
@@ -246,8 +247,9 @@ def run_reference_cuda(args):
 
 # ------------------------------------------------------------------------------------------------ our arm
 def measure_config(env_name, N, T, steps, warmup, dev, rank, world, dist, e2e_mode="graph", comm_floats=0,
-                   ncu_range=False, ncu_range_e2e=False, clocks=None, tape_dtype="fp32"):
-    """Kernel path + end-to-end numbers of one workload on this rank.  Returns a dict of raw timings and geometry.
+                   ncu_range=False, ncu_range_e2e=False, clocks=None, tape_dtype="fp32", keep_outputs=False):
+    """Kernel path + end-to-end numbers of one workload on this rank.  Returns a dict of raw timings and geometry (with
+    keep_outputs, under "outputs": what the last timed rollout of each path returned, as host arrays).
     tape_dtype "bf16": the adjoint tape stores (v, a, f_tot) of every row as bf16 (BASELINE config C2 "bf16 states"; arithmetic
     and the state stay fp32)."""
     import torch
@@ -307,7 +309,7 @@ def measure_config(env_name, N, T, steps, warmup, dev, rank, world, dist, e2e_mo
         if record:
             ev3[2].record()
             phase_events.append(ev3)
-        return gq
+        return dict(q=q, qd=qd, gq=gq, gqd=gqd, gact=gact, gmusc=gm)
 
     for _ in range(warmup):
         kernel_rollout()
@@ -321,7 +323,7 @@ def measure_config(env_name, N, T, steps, warmup, dev, rank, world, dist, e2e_mo
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     ev[0].record()
     for _ in range(steps):
-        kernel_rollout(record=True)
+        last = kernel_rollout(record=True)
     ev[1].record()
     barrier()
     kernel_ms = ev[0].elapsed_time(ev[1])
@@ -363,7 +365,7 @@ def measure_config(env_name, N, T, steps, warmup, dev, rank, world, dist, e2e_mo
         torch.cuda.current_stream().synchronize()
         return float(host_loss)
 
-    e2e_steps = max(1, steps // 2)
+    e2e_steps = steps
     for _ in range(max(1, warmup // 2)):
         e2e_rollout()
     barrier()
@@ -395,7 +397,7 @@ def measure_config(env_name, N, T, steps, warmup, dev, rank, world, dist, e2e_mo
         for _ in range(max(1, warmup // 2)):
             graphed_rollout()
         barrier()
-        if ncu_range_e2e:          # launch list of ONE end-to-end rollout (profiles/): ncu --profile-from-start off
+        if ncu_range_e2e:          # launch list of ONE end-to-end rollout: ncu --profile-from-start off
             torch.cuda.profiler.start()
             graphed_rollout()
             torch.cuda.synchronize()
@@ -407,6 +409,7 @@ def measure_config(env_name, N, T, steps, warmup, dev, rank, world, dist, e2e_mo
         barrier()
         e2e_ms = e3[0].elapsed_time(e3[1])
         e2e_api = "diffrl_b200.rollout.GraphedRollout(envs.%s): one CUDA graph = H2D actions + %d x env.step + backward + D2H" % (env_name, T)
+        host_loss, host_grad = roll.host_loss, roll.host_grad
         del roll
 
     tile = int(lib.dfx_pack_query(eng.pack, 9))
@@ -415,14 +418,17 @@ def measure_config(env_name, N, T, steps, warmup, dev, rank, world, dist, e2e_mo
                eager_ms=eager_ms, fwd_ms=fwd_ms, bwd_ms=bwd_ms, launches=int(launches), steps=steps, e2e_steps=e2e_steps,
                tape_mb=tape_mb, tape_dtype=tape_dtype, e2e_api=e2e_api, h2d=int(host_actions.numel() * 4), d2h=int(host_grad.numel() * 4 + 4),
                comm_floats=comm_floats if comm is not None else 0)
-    del env, eng, acts, muscs, host_actions, host_grad
+    if keep_outputs:
+        out["outputs"] = {"kernel_" + k: v.detach().cpu().numpy() for k, v in last.items() if v is not None}
+        out["outputs"].update(e2e_loss=host_loss.numpy().reshape(1).copy(), e2e_grad_actions=host_grad.numpy().copy())
+    del env, eng, acts, muscs, host_actions, host_grad, last
     import gc
     gc.collect()
     torch.cuda.empty_cache()
     return out
 
 
-def roofline_record(m, peaks, peak_kind, traffic=None, fp32=None):
+def roofline_record(m, peaks, peak_kind):
     """SURVEY.md section 8d roofline of the adjoint launch (+ the forward launch and the design's own bytes beside it)."""
     N, Q, D, A, S, mm = m["N"], m["Q"], m["D"], m["D"] + m["M"], m["S"], m["mm"]
     s_fwd, s_bwd = algorithmic_bytes(Q, D, A, S)
@@ -433,7 +439,7 @@ def roofline_record(m, peaks, peak_kind, traffic=None, fp32=None):
     whole = N * (s_fwd + s_bwd) / ((m["fwd_ms"] + m["bwd_ms"]) * 1e-3) / 1e9
     family = ("dfx_tile_kernel<BWD=1> (adjoint of one env-step, %d-environment tiles, TMA bulk tape copies)" % m["tile"]) if m["tile"] \
         else "dfx_step_kernel<G,BWD=1> (adjoint of one env-step, lane groups)"
-    return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
+    return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
             "peak_source": peak_kind, "kernel": family,
             "algorithmic_bytes_per_launch": N * s_bwd,
             "bytes_definition": "SURVEY.md section 8d, state-only tape: %d B forward + %d B adjoint per env-step" % (s_fwd, s_bwd),
@@ -442,33 +448,8 @@ def roofline_record(m, peaks, peak_kind, traffic=None, fp32=None):
             "env_step_fwd_plus_adjoint": {"achieved": whole, "frac": whole / peak},
             "design_frac": dach / peak, "design_achieved": dach, "design_bytes_per_launch": N * d_bwd,
             "design_bytes_definition": "what this design moves: tape rows with the forward intermediates (4 x %d B per env-substep) + H^-1 blocks + state I/O" % m["row"],
-            "fp32": fp32,
-            "note": "the fused path is FP32-issue / latency bound, not HBM bound (profiles/, DESIGN.md section 3); launch durations are "
+            "note": "the fused path is FP32-issue / latency bound, not HBM bound (DESIGN.md section 3); launch durations are "
                     "averages over the timed rollouts (CUDA events on the launching stream)"}
-
-
-def profile_numbers(env_name, N, m, sm_mhz):
-    """(DRAM bytes per adjoint launch, fp32 record) from the committed ncu capture of this launch shape (profiles/r0X_traffic.json,
-    tools/make_traffic_json.py), or (None, None) when no capture of this (env, num_envs) is committed."""
-    for tname in ("r02_traffic.json", "r01_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", tname)
-        if not os.path.exists(tpath):
-            continue
-        with open(tpath) as f:
-            prof = json.load(f).get(env_name, {})
-        if not prof or prof.get("num_envs", 4096) != N:
-            continue
-        fp32 = None
-        if "bwd_fp32_flop_per_launch" in prof:
-            # SURVEY.md 8d's second yardstick: fp32 FLOP actually executed (counted by ncu for this launch shape) per
-            # second against the CUDA-core peak 148 SMs x 128 lanes x 2 FLOP x the SM clock sampled during the run
-            flop = prof["fwd_fp32_flop_per_launch"] + prof["bwd_fp32_flop_per_launch"]
-            peak = 148 * 128 * 2 * sm_mhz * 1e6
-            secs = (m["fwd_ms"] + m["bwd_ms"]) * 1e-3
-            fp32 = {"achieved_tflops": flop / secs / 1e12, "peak_tflops": peak / 1e12, "frac": flop / secs / peak,
-                    "flop_per_env_step": flop / N, "source": "profiles/%s (ncu instruction counts)" % tname}
-        return prof.get("bwd_dram_bytes_per_launch"), fp32
-    return None, None
 
 
 def config_record(m, world, peaks, peak_kind):
@@ -482,7 +463,7 @@ def config_record(m, world, peaks, peak_kind):
             "kernel_family": ("tile (%d envs per CTA)" % m["tile"]) if m["tile"] else "lane group",
             "tape_mb_per_rollout": m["tape_mb"], "tape_storage": "fp32" if m.get("tape_dtype", "fp32") == "fp32" else "bf16 for (v, a, f_tot) of every row, fp32 otherwise (arithmetic fp32)",
             "gpu_launches": m["launches"],
-            "roofline": roofline_record(m, peaks, peak_kind, *profile_numbers(m["env"], m["N"], m, 1965.0))}
+            "roofline": roofline_record(m, peaks, peak_kind)}
 
 
 def run_ours(args):
@@ -503,16 +484,19 @@ def run_ours(args):
     comm_floats = 16384     # the Ant actor's flattened gradient (cfg/shac/ant.yaml); one all-reduce per rollout when world > 1
     with ClockSampler(local) as clocks:
         head = measure_config(env_name, N, T, args.steps, args.warmup, dev, rank, world, dist, e2e_mode=args.e2e,
-                              comm_floats=comm_floats, ncu_range=args.ncu_range, ncu_range_e2e=args.ncu_range_e2e)
+                              comm_floats=comm_floats, ncu_range=args.ncu_range, ncu_range_e2e=args.ncu_range_e2e,
+                              keep_outputs=bool(args.dump_outputs) and rank == 0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, head.pop("outputs"))
     # ---- the other named configs (BASELINE.json): short runs, same measurement
     subs = {}
     if not args.no_configs:
         plan = []
         if world > 1:
-            plan.append(("c4", "AntEnv", 8192, 32, max(2, args.steps // 2), 2))
+            plan.append(("c4", "AntEnv", 8192, 32, args.steps, 2))
         else:
-            plan += [("humanoid8192", "HumanoidEnv", 8192, 32, 2, 1), ("humanoid8192_bf16_tape", "HumanoidEnv", 8192, 32, 2, 1),
-                     ("snu4096_bptt128", "SNUHumanoidEnv", 4096, 128, 2, 1), ("cartpole64", "CartPoleSwingUpEnv", 64, 32, 4, 2)]
+            plan += [("humanoid8192", "HumanoidEnv", 8192, 32, args.steps, 1), ("humanoid8192_bf16_tape", "HumanoidEnv", 8192, 32, args.steps, 1),
+                     ("snu4096_bptt128", "SNUHumanoidEnv", 4096, 128, args.steps, 1), ("cartpole64", "CartPoleSwingUpEnv", 64, 32, args.steps, 2)]
         for key, e, n, t, k, w in plan:
             try:
                 subs[key] = measure_config(e, n, t, k, w, dev, rank, world, dist, e2e_mode=args.e2e, comm_floats=comm_floats,
@@ -540,7 +524,7 @@ def run_ours(args):
     peaks, peak_kind = measured_peaks()
     value = world * N * T * args.steps / (head["kernel_ms"] * 1e-3)
     e2e_value = world * N * T * head["e2e_steps"] / (head["e2e_ms"] * 1e-3)
-    traffic, fp32 = profile_numbers(env_name, N, head, clocks.summary().get("sm_mhz") or 1965.0)
+    l2_mb = torch.cuda.get_device_properties(dev).L2_cache_size / 1e6
     line = {
         "metric": METRIC, "value": value, "unit": "env-steps/s", "n_gpus": world,
         "value_is": "kernel path: simulation-kernel launches only, inputs resident (the headline is e2e)",
@@ -549,14 +533,14 @@ def run_ours(args):
         "config": {"workload": "%s num_envs=%d/GPU SHAC short-horizon=%d (rollout forward + adjoint), substeps=%d, "
                                "mass_matrix_freq=%d" % (env_name, N, T, head["S"], head["mm"]),
                    "parallelism": "env-sharded x%d, no data-path collective%s" % (world, "; one %d KB policy-gradient all-reduce per rollout (e2e)" % (comm_floats * 4 // 1024) if world > 1 else ""),
-                   "cache": "per-rollout tape %.0f MB > 126 MB L2 (inputs larger than L2)" % head["tape_mb"],
+                   "cache": "per-rollout tape %.0f MB vs %.0f MB L2" % (head["tape_mb"], l2_mb),
                    "kernel_family": ("tile (%d envs per CTA, TMA tape copies)" % head["tile"]) if head["tile"] else "lane group"},
         "e2e": {"value": e2e_value, "unit": "env-steps/s", "h2d_bytes_per_step": head["h2d"], "d2h_bytes_per_step": head["d2h"],
                 "api": head["e2e_api"], "ms_per_step": head["e2e_ms"] / head["e2e_steps"],
                 "eager_env_step_loop": {"value": world * N * T * head["e2e_steps"] / (head["eager_ms"] * 1e-3), "ms_per_step": head["eager_ms"] / head["e2e_steps"]}},
         "gpu_launches": head["launches"],
         "kernel_ms": {"forward_env_step": head["fwd_ms"], "backward_env_step": head["bwd_ms"]},
-        "roofline": roofline_record(head, peaks, peak_kind, traffic, fp32),
+        "roofline": roofline_record(head, peaks, peak_kind),
         "clocks": clocks.summary(),
     }
     if subs:
@@ -571,6 +555,23 @@ def run_ours(args):
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_ARRAY_BYTES = 7 << 20      # larger arrays are stored as a seeded row sample: the 8 arrays stay under 64 MB
+
+
+def dump_outputs(path, outputs):
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for name, a in outputs.items():
+        a = np.asarray(a, dtype=np.float32)
+        if a.nbytes > DUMP_ARRAY_BYTES:
+            rows = a.reshape(a.shape[0], -1)
+            keep = max(1, rows.shape[0] * DUMP_ARRAY_BYTES // a.nbytes)
+            idx = np.sort(np.random.default_rng(0).choice(rows.shape[0], keep, replace=False))
+            np.save(os.path.join(path, name + "_rows.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def main():
@@ -591,6 +592,8 @@ def main():
                     help="wrap one graphed end-to-end rollout in cudaProfilerStart/Stop (for ncu --profile-from-start off)")
     ap.add_argument("--ncu-range", action="store_true",
                     help="wrap ONE kernel-path step in cudaProfilerStart/Stop (use with ncu --profile-from-start off)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the headline config's last timed rollout returned as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-"""Drop-in ``dflex`` package: ``import dflex as df`` resolves to the B200-native implementation in
+"""Drop-in ``dflex`` package: ``import dflex as df`` resolves to the H100-native implementation in
 ``diffrl_b200.dflex_api`` (same import surface as NVlabs/DiffRL's ``dflex``), so the reference's
 ``envs/*.py``, ``utils/load_utils.py`` and ``algorithms/*.py`` run on it unchanged."""
 import sys as _sys

@@ -27,7 +27,7 @@ def lib():
     if not os.path.isfile(LIB_PATH):
         raise DfxError(
             "diffrl_b200: CUDA library %s not found. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback for the simulation step." % LIB_PATH)
+            "(nvcc, sm_90a). There is no CPU fallback for the simulation step." % LIB_PATH)
     try:
         L = ctypes.CDLL(LIB_PATH)
     except OSError as exc:  # e.g. libcudart missing

@@ -364,8 +364,7 @@ __device__ __forceinline__ void planar_transition_backward_env(const DfxPlanarPa
 // =====================================================================================
 // The transition of a whole TILE of E environments by all NT threads of its CTA (dfx_tile.cu: the epilogue of the simulation
 // launch and the prologue of the adjoint launch of dfx_env_step_forward / _backward).  One thread per environment alone is slow
-// as an epilogue -- ~150 dependent, uncoalesced global accesses by a single warp (~9 us, as long as the stand-alone launch it
-// replaces) -- so the rows are STAGED in the (dead) scratch tile: thread e < E evaluates environment e entirely in shared memory,
+// as an epilogue -- ~150 dependent, uncoalesced global accesses by a single warp -- so the rows are STAGED in the (dead) scratch tile: thread e < E evaluates environment e entirely in shared memory,
 // and all NT threads move the rows between the tile and global memory, element k of environment e by thread k * E + e
 // (conflict-free scratch accesses).  Same per-environment arithmetic as above.
 // =====================================================================================

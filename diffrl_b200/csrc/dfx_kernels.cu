@@ -1,5 +1,5 @@
 // dfx_kernels.cu -- the C ABI (include/dfx.h) of the differentiable articulated rigid-body step and the
-// LANE-GROUP sm_100a kernels (the humanoids and any generic articulation; the small DiffRL articulations run
+// LANE-GROUP sm_90a kernels (the humanoids and any generic articulation; the small DiffRL articulations run
 // on the 32-environment tile kernels of dfx_tile.cu, same phase code, other mapping).
 //
 // Execution model here: a cooperative group of G lanes (8, 16 or 32; a sub-warp tile) owns one
@@ -236,7 +236,7 @@ static void set_err(char* err, int n, const std::string& m) {
 
 extern "C" {
 
-const char* dfx_version(void) { return "diffrl_b200 dfx 0.2 (sm_100a)"; }
+const char* dfx_version(void) { return "diffrl_b200 dfx 0.2 (sm_90a)"; }
 int dfx_tile_joint_mask(int L, int D, int Q, int C, int M) { return tile_joint_mask(L, D, Q, C, M); }
 int dfx_abi_sizeof(int which) {
     switch (which) {

@@ -158,7 +158,7 @@ DFX_HD bool is_joint(const Pack& P, int type, int t) { return ((P.jmask >> t) & 
 // articulation holds 1-4 links, so a lane group of 16 or 32 runs it with most lanes idle; cta_tasks() instead spreads
 // the (link, environment) pairs of ALL the environments of the CTA over consecutive threads, link-major: a level
 // is then typically ONE warp with full lanes, uniform joint types and broadcast pack reads, at the price of a
-// CTA-wide barrier per level.  Measured (same box, Ant 4096): adjoint -8.5 %; the light forward recursions (one
+// CTA-wide barrier per level.  The adjoint recursions gain from it; the light forward recursions (one
 // transform product or two vector adds per level) lose more to the barriers than they gain and stay per group.
 template <class Grp, class F>
 DFX_HD void level_tasks(const Pack& P, SP s, int lev, bool lead, const Grp& g, F f) {
@@ -700,7 +700,7 @@ DFX_HD void body_force_adj(const Pack& P, const Layout& Y, SP s, const Grp& g) {
 }
 
 // =====================================================================================
-// Deterministic scatter-adds.  Shared memory on sm_100 has native atomics for 32-bit integers only: atomicAdd(float*)
+// Deterministic scatter-adds.  Shared memory on sm_90 has native atomics for 32-bit integers only: atomicAdd(float*)
 // and the 64-bit integer atomicAdd both compile to ATOMS.CAST.SPIN compare-and-swap loops, which serialise badly when
 // many lanes hit one body (152 muscles on 11 bodies: 69 % of all stall samples).  Integer adds are also associative,
 // so a fixed-point sum is bit-reproducible whatever the order.  A contribution x is scaled by a power of two, rounded
@@ -921,8 +921,7 @@ DFX_HD void contact_point_adj(const Pack& P, const Layout& Y, SP s, int k, float
         fx_scatter(sp_int(s + Y.av) + b * 6, hi + P.L * 7 + b * 6, poison, b, c6, scale, g);
     } else {
         // contact-only models: at most a handful of penetrating points share a body, and the compare-and-swap
-        // float add is then 8-12 % cheaper for the whole adjoint than fixed point + read-back (same-box A/B, Ant
-        // and Humanoid).  The order of these few adds is not fixed, so the last bits of the gradient may vary.
+        // float add is then cheaper for the whole adjoint than fixed point + read-back (Ant and Humanoid).  The order of these few adds is not fixed, so the last bits of the gradient may vary.
         const SP ax = s + Y.aXsc + b * 7;
         const SP avp = s + Y.av + b * 6;
 #pragma unroll
@@ -1696,7 +1695,7 @@ DFX_HD void substep_adj(const Pack& P, const Layout& Y, SP s, float dt, bool app
     zero_range(s + Y.aIbar, P.L * 12, g);
     // (no barrier: integrate_adj and solve_adj do not touch the zeroed accumulators, and two barriers follow before their first use)
     // phase_sync(): CTA-wide barrier that keeps the warps of a CTA inside the same phase, so that the
-    // instruction working set per SM is one or two phases (~10 KB each) instead of the whole 140 KB body
+    // instruction working set per SM is one or two phases instead of the whole body
     integrate_adj(P, Y, s, dt, g);
     solve_adj(P, Y, s, hv, g);              // tau slot <- atau
     g.copy_wait_all();                      // the bulk of the tape row (transforms, S, v, a, wrenches) is needed from here on

@@ -1,4 +1,4 @@
-// dfx_tile.cu -- E-environment tile kernels of the differentiable articulated rigid-body step (sm_100a).
+// dfx_tile.cu -- E-environment tile kernels of the differentiable articulated rigid-body step (sm_90a).
 //
 // This translation unit is compiled once per tile width:  nvcc -DDFX_TILE_E=E -Ddfx=dfx_eE  with E = 8, 16, 32
 // (the namespace is renamed per build so that the three instantiations of the shared headers do not collide).

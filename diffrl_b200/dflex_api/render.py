@@ -9,4 +9,4 @@ class UsdRenderer:
         except ImportError as exc:
             raise ImportError("UsdRenderer needs the `pxr` (usd-core) package, which is not installed; "
                               "construct environments with render=False") from exc
-        raise NotImplementedError("USD rendering is not part of the B200 hot-path package")
+        raise NotImplementedError("USD rendering is not part of the hot-path package")

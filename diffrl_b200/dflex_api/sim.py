@@ -4,7 +4,7 @@
 signature and semantics of the reference (``dflex/dflex/sim.py:2182-2221``): ``substeps`` symplectic-Euler
 substeps of ``dt/substeps`` with the actuation held constant, the joint-space inertia re-factorised
 every ``mass_matrix_freq`` substeps, gradients flowing to ``state_in.joint_q / joint_qd / joint_act``
-and ``model.muscle_activation``.  Underneath, one fused sm_100a kernel per env-step (and one for its
+and ``model.muscle_activation``.  Underneath, one fused sm_90a kernel per env-step (and one for its
 adjoint) replaces the reference's tape of 10-11 generated kernels per substep.
 """
 import torch

@@ -3,7 +3,7 @@
 The reference stores every Model tensor tiled over the environments (``dflex/dflex/model.py:1646-1879``:
 env ``e``'s links are rows ``e*L .. e*L+L-1``, ``joint_parent`` / ``contact_body0`` /
 ``contact_material`` / ``muscle_links`` are GLOBAL indices).  All environments of a DFlexEnv are copies
-of one articulation (``envs/ant.py:97-124`` with ``env_dist = 0``), so the B200 kernels take the
+of one articulation (``envs/ant.py:97-124`` with ``env_dist = 0``), so the kernels take the
 description of ONE articulation and share it across the batch.  This module slices environment 0 out
 of the tiled tensors, makes the indices env-local, and checks that every other environment is
 identical (raising otherwise: heterogeneous batches are not supported by the fused kernels).

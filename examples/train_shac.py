@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Short-Horizon Actor-Critic (SHAC) on the B200-native differentiable simulator -- example trainer.
+"""Short-Horizon Actor-Critic (SHAC) on the H100-native differentiable simulator -- example trainer.
 
 The reference's ``algorithms/shac.py`` runs unchanged on the drop-in ``dflex`` package (INTEGRATION.md); this
 file is an independently written, vectorised restatement of the same algorithm (Xu et al., ICLR 2022;

@@ -1,4 +1,4 @@
-/* dfx.h -- C ABI of the B200-native differentiable articulated rigid-body step.
+/* dfx.h -- C ABI of the H100-native (sm_90a) differentiable articulated rigid-body step.
  *
  * This is the drop-in boundary underneath `dflex.sim.SemiImplicitIntegrator.forward`
  * (reference NVlabs/DiffRL dflex/dflex/sim.py:2182).  In the reference that call fans out into

@@ -10,7 +10,7 @@ What lands in ``baseline/_ref/`` (never in git history; shipped by gpurun like t
   NON-NUMERICAL edits listed in ``PATCHES`` below and nothing else;
 * ``envs/ utils/ algorithms/ models/ examples/cfg/``   byte-for-byte copies;
 * ``refdflex/dflex/kernels/``   the reference's generated C++/CUDA kernels, built HERE by the reference's own
-  ``compile()`` (cross-compiled for sm_100; the reference ships ``compute_35`` PTX only, which nvcc 12.9 rejects).
+  ``compile()`` (cross-compiled for sm_90; the reference ships ``compute_35`` PTX only, which nvcc 12.9 rejects).
 
 Two things use it, both on the GPU box:
 
@@ -34,8 +34,8 @@ DST = os.path.join(ROOT, "baseline", "_ref")
 PATCHES = [
     ("adjoint.py", "node.slice.value", "node.slice",
      "ast.Index no longer wraps subscripts (Python >= 3.9)"),
-    ("adjoint.py", "-gencode=arch=compute_35,code=compute_35", "-gencode=arch=compute_100,code=sm_100",
-     "adjoint.py:1861: nvcc 12.9 has no compute_35; build the generated kernels for the B200"),
+    ("adjoint.py", "-gencode=arch=compute_35,code=compute_35", "-gencode=arch=compute_90,code=sm_90",
+     "adjoint.py:1861: nvcc 12.9 has no compute_35; build the generated kernels for the H100"),
     ("adjoint.py", "    use_cuda = torch.cuda.is_available()\n",
      "    use_cuda = torch.cuda.is_available() or os.environ.get('DFLEX_FORCE_CUDA_BUILD') == '1'\n",
      "adjoint.py:1750: allow cross-compiling the CUDA module in the GPU-less build container"),
@@ -92,7 +92,7 @@ def install(with_cuda=True):
     env = dict(os.environ)
     env["DFLEX_FORCE_CUDA_BUILD"] = "1" if with_cuda else "0"
     env.setdefault("CUDA_HOME", "/usr/local/cuda")
-    env["TORCH_CUDA_ARCH_LIST"] = "10.0"
+    env["TORCH_CUDA_ARCH_LIST"] = "9.0"
     env.setdefault("MAX_JOBS", "8")
     code = ("import sys, numpy as np; np.Inf = np.inf; sys.path[:0] = [%r, %r, %r]; import dflex; print('reference dflex built:', dflex.__file__)"
             % (os.path.join(HERE, "refshim"), os.path.join(DST, "refdflex"), DST))

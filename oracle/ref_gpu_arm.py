@@ -7,7 +7,7 @@ package, not to this repo's) on the git-ignored install made by ``oracle/install
     python oracle/ref_gpu_arm.py --env AntEnv --num-envs 4096 --horizon 32 --rollouts 2 --warmup 1 [--device cuda:0|cpu]
 
 ``--device cuda:0``: the reference's CUDA codegen path (``dflex/dflex/adjoint.py:1247-1262`` launch templates), rebuilt
-for sm_100 with the ONE flag edit at ``adjoint.py:1861`` (``compute_35`` -> ``compute_100``) -- SURVEY.md section 8d's
+for sm_90 with the ONE flag edit at ``adjoint.py:1861`` (``compute_35`` -> ``compute_90``) -- SURVEY.md section 8d's
 "second bar", the only pre-existing GPU implementation of this path.
 ``--device cpu``: the reference's CPU path (a serial loop, ``adjoint.py:1271-1279``).
 
@@ -47,7 +47,7 @@ def main():
     if a.device == "cpu":
         os.environ["CUDA_VISIBLE_DEVICES"] = ""
     # the reference caches its generated kernels by comparing source strings, and the source differs with / without the CUDA
-    # half: always generate both, so that the ONE prebuilt kernels.so (CPU + sm_100) is reused on every box and device
+    # half: always generate both, so that the ONE prebuilt kernels.so (CPU + sm_90) is reused on every box and device
     os.environ["DFLEX_FORCE_CUDA_BUILD"] = "1"
     import torch
     import dflex  # noqa: F401  (the reference's; loads its prebuilt kernels.so)
@@ -96,7 +96,7 @@ def main():
     out = {"impl": "reference", "device": a.device, "env": a.env, "num_envs": a.num_envs, "horizon": a.horizon,
            "rollouts": a.rollouts, "forward_s": tf, "backward_s": tb, "env_steps_per_s": steps / (tf + tb),
            "loss": loss, "grad_abs_sum": gsum, "finite": bool(np.isfinite(loss) and np.isfinite(gsum)),
-           "api": "reference envs.%s.step -> reference dflex.sim.SemiImplicitIntegrator (%s codegen kernels)" % (a.env, "CUDA sm_100" if cuda else "CPU"),
+           "api": "reference envs.%s.step -> reference dflex.sim.SemiImplicitIntegrator (%s codegen kernels)" % (a.env, "CUDA sm_90" if cuda else "CPU"),
            "peak_mem_gb": (torch.cuda.max_memory_allocated() / 1e9) if cuda else None}
     if a.stamp:
         out["t_start"], out["t_end"] = t_start, t_end

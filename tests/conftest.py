@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a: pytest -m gpu)")
 
 
 ENVS = ["CartPoleSwingUpEnv", "AntEnv", "HumanoidEnv", "SNUHumanoidEnv", "HopperEnv", "CheetahEnv"]

@@ -177,8 +177,11 @@ def test_non_finite_contribution_poisons_the_sum():
 
 
 def test_launch_plan_keeps_a_full_wave_of_ant_resident():
-    """4096 Ant environments fit one wave of CTAs on 148 SMs (forward and adjoint): DESIGN.md section 4."""
+    """4096 Ant environments fit one wave of CTAs on the device's SMs (132 on an H100 SXM; forward and adjoint): DESIGN.md
+    section 4."""
+    import torch
     from diffrl_b200.engine import ArticulationEngine
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
     d, emu, *_ = _case("AntEnv", 1)
     eng = ArticulationEngine(emu.desc, 1, "cuda:0")
     for bwd in (0, 1):
@@ -186,7 +189,7 @@ def test_launch_plan_keeps_a_full_wave_of_ant_resident():
         assert eng.lib.dfx_launch_plan(eng.pack, bwd, out) == 0
         lanes, envs_per_cta, ctas_per_sm, smem, stride, pack = list(out)
         assert (lanes, envs_per_cta) == (32, 32)          # tile kernel: one CTA = 32 environments, lane = environment
-        assert envs_per_cta * ctas_per_sm * 148 >= 4096
+        assert envs_per_cta * ctas_per_sm * sms >= 4096
         assert smem == pack + envs_per_cta * stride * 4 and (smem + 1024) * ctas_per_sm <= 227 * 1024
 
 
@@ -252,7 +255,7 @@ def test_launch_plan_keeps_sixteen_humanoids_per_sm(name, width):
     """The large articulations run on the compact scratch layouts (csrc/dfx_pack.h: mass-matrix temporaries overlaid on
     the per-substep temporaries, H^-1 read from the tape by the adjoint) so that 16 environments stay resident per SM,
     forward and adjoint: the Humanoid as two 8-environment CTAs that hide each other's barrier waits, the SNU model as
-    one 16-environment CTA of 16 warps (its 152 muscles fill the item slots; measured 7 % faster, DESIGN.md section 3)."""
+    one 16-environment CTA of 16 warps (its 152 muscles fill the item slots, DESIGN.md section 3)."""
     from diffrl_b200.engine import ArticulationEngine
     d, model = load_golden(name)
     eng = ArticulationEngine.from_model(model, "cuda:0", int(d["meta/num_envs"]))

@@ -14,8 +14,8 @@ FWD_RTOL = 1e-5
 GRAD_RTOL = 5e-5
 _ILL_CONDITIONED = {"HumanoidEnv": 3e-5, "SNUHumanoidEnv": 3e-5}
 # ON THE REFERENCE'S GOLDEN CASES themselves (tests/golden, unperturbed states) the bar is the north-star's 1e-5 for every
-# model but SNU: measured Humanoid 6.8e-6, SNU 1.15e-5 on the B200.  The host-emulation A/B (tests/test_emu_golden.py::
-# test_explicit_inverse_is_not_the_parity_floor) shows where SNU's last 15 % comes from: FMA contraction (8.9e-6 without,
+# model but SNU: measured Humanoid 6.8e-6, SNU 1.3e-5 on an H100.  The host-emulation A/B (tests/test_emu_golden.py::
+# test_explicit_inverse_is_not_the_parity_floor) shows where SNU's excess over 1e-5 comes from: FMA contraction (8.9e-6 without,
 # 1.2e-5 with), not the explicit H^-1 (8.9e-6 vs 8.0e-6 with the reference's triangular sweeps).
 _GOLDEN = {"SNUHumanoidEnv": 1.5e-5}
 

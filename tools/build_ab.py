@@ -17,5 +17,5 @@ for name, src, flags in g.UNITS:
 assert all(p.wait() == 0 for p in procs)
 os.makedirs(os.path.join(ROOT, "build", "ablib"), exist_ok=True)
 out = os.path.join(ROOT, "build", "ablib", "libdfx_%s.so" % tag)
-subprocess.check_call([nvcc, "-arch=sm_100a", "-shared", "-o", out] + objs, cwd=ROOT)
+subprocess.check_call([nvcc, "-arch=sm_90a", "-shared", "-o", out] + objs, cwd=ROOT)
 print(out)

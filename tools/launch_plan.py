@@ -15,5 +15,5 @@ for name in ["CartPoleSwingUpEnv", "HopperEnv", "CheetahEnv", "AntEnv", "Humanoi
         out = (ctypes.c_int * 6)()
         eng.lib.dfx_launch_plan(eng.pack, bwd, out)
         g, e, c, smem, stride, pack = list(out)
-        print("%-20s %s lanes/env %2d envs/CTA %2d CTAs/SM %2d -> %3d envs/SM (%6d on 148 SMs)  smem/CTA %6d B  scratch %5d B/env  pack %5d B"
+        print("%-20s %s lanes/env %2d envs/CTA %2d CTAs/SM %2d -> %3d envs/SM (%6d on 132 SMs)  smem/CTA %6d B  scratch %5d B/env  pack %5d B"
               % (name, "bwd" if bwd else "fwd", g, e, c, e * c, e * c * 148, smem, stride * 4, pack))

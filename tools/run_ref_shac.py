@@ -3,7 +3,7 @@
     python tools/run_ref_shac.py --dflex ours|reference --env ant --seed 0 --max-epochs 2000 --device cuda:0 --out curve.json
 
 ``--dflex ours``: this repo's drop-in package (the claim: the trainer runs unchanged on it); ``--dflex reference``: the
-reference's own dflex (its CUDA codegen rebuilt for sm_100, or its CPU path with ``--device cpu``).  The training curve
+reference's own dflex (its CUDA codegen rebuilt for sm_90, or its CPU path with ``--device cpu``).  The training curve
 (policy loss per epoch = minus the mean undiscounted return estimate the trainer logs, episode returns) is written as JSON.
 Harness only: the trainer file is byte-identical to the reference's; ``oracle/refshim/torch_compat.py`` supplies the
 torch >= 2 indexing behaviour it was written against.
