@@ -56,6 +56,14 @@ def lib():
                                               _F, _F, ctypes.POINTER(DfxActionMap), _F, _F, _F, _F, _F, _F, ctypes.c_void_p]
         L.dfx_step_backward_mapped.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
                                                ctypes.POINTER(DfxActionMap), _F, _F, _F, _F, _F, _F, _F, _F, _F, ctypes.c_void_p]
+    if hasattr(L, "dfx_step_backward_recompute"):     # recompute adjoint (include/dfx.h); env-step entry: env_ops._bind
+        L.dfx_recompute_workspace_floats.restype = ctypes.c_longlong
+        L.dfx_recompute_workspace_floats.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+        L.dfx_step_backward_recompute.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
+                                                  _F, _F, _F, _F, _F, _F, _F, _F, _F, _F, _F, ctypes.c_void_p]
+        L.dfx_step_backward_mapped_recompute.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
+                                                         _F, _F, ctypes.POINTER(DfxActionMap), _F, _F, _F, _F, _F, _F, _F, _F, _F,
+                                                         ctypes.c_void_p]
     if os.environ.get("DFX_FLAGS"):      # tuning flags of include/dfx.h (A/B runs of the test-suite)
         L.dfx_set_flags(int(os.environ["DFX_FLAGS"]))
     _lib = L

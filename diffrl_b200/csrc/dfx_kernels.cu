@@ -628,4 +628,115 @@ int dfx_env_step_backward(const dfx_pack_t* p, int n, int substeps, int mm_freq,
     return run_step(p, a, true, stream);
 }
 
+// ---- recompute adjoint (include/dfx.h dfx_*_backward_recompute): no stored tape, the env-step's forward is re-run from its
+// input state into a one-env-step workspace right before the adjoint reads it
+long long dfx_recompute_workspace_floats(const dfx_pack_t* p, int n, int substeps, int mm_freq) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0) return -1;
+    return dfx_tape_floats(p, n, substeps, mm_freq) + (long long)n * (p->header.Q + p->header.D);
+}
+
+// end state of the recomputed forward: the workspace's tail, q [n*Q] then qd [n*D]
+static float* workspace_q_end(const dfx_pack_t* p, const StepArgs& a, float* ws) { return ws + dfx_tape_floats(p, a.N, a.substeps, a.mm_freq); }
+
+// one launch on the tile kernels: the forward into the workspace, the barrier sequence of dfx_tile_recompute_kernel, the adjoint.
+// `a` holds the adjoint's arguments (as the stored-tape entry would launch them); the forward's are added here.
+static int run_recompute_fused(const dfx_pack_t* p, StepArgs& a, const float* q, const float* qd, float* ws, void* stream) {
+    a.q = q; a.qd = qd;
+    a.q_out = workspace_q_end(p, a, ws); a.qd_out = a.q_out + (long long)a.N * p->header.Q;
+    a.tape = ws; a.tape_in = ws;
+    a.used = nullptr; a.has_derived = 0;
+    a.hinv_base = tape_geom(p->header.L, p->header.Q, p->header.D, tape_envs(p, a.N), a.substeps, a.mm_freq, p->bf16 != 0).hinv_base;
+    a.tape_bf16 = p->bf16;
+    a.flags = g_flags;
+    KernelArgs ka;
+    ka.header = p->header;
+    ka.blob = p->blob;
+    ka.step = a;
+    int e = (int)cudaErrorInvalidConfiguration;
+    switch (p->tile) {
+        case 8: e = dfx_tile_launch_recompute_e8(&ka, stream); break;
+        case 16: e = dfx_tile_launch_recompute_e16(&ka, stream); break;
+        case 32: e = dfx_tile_launch_recompute_e32(&ka, stream); break;
+    }
+    g_launches.fetch_add(1);
+    return e;
+}
+
+// the fused kernel exists for every tile pack; the A/B variants of flag bit 6 have none (two launches instead)
+static bool recompute_fuses(const dfx_pack_t* p) { return p->tile != 0 && !(g_flags & 64); }
+
+int dfx_step_backward_recompute(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                                const float* q, const float* qd, const float* act, const float* musc, float* workspace,
+                                const float* gq_out, const float* gqd_out,
+                                float* gq, float* gqd, float* gact, float* gmusc, void* stream) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !act) return (int)cudaErrorInvalidValue;
+    if (p->header.M > 0 && !musc) return (int)cudaErrorInvalidValue;
+    StepArgs a;
+    memset(&a, 0, sizeof a);
+    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
+    a.dt_sub = (float)(dt / (double)substeps);
+    if (!recompute_fuses(p)) {
+        float* q_end = workspace_q_end(p, a, workspace);
+        const int e = dfx_step_forward(p, n, substeps, mm_freq, dt, q, qd, act, musc, q_end, q_end + (long long)n * p->header.Q, workspace, nullptr, stream);
+        if (e != 0) return e;
+        return dfx_step_backward(p, n, substeps, mm_freq, dt, act, musc, workspace, gq_out, gqd_out, gq, gqd, gact, gmusc, stream);
+    }
+    a.act = act; a.musc = musc; a.gq_out = gq_out; a.gqd_out = gqd_out;
+    a.gq = gq; a.gqd = gqd; a.gact = gact; a.gmusc = gmusc;
+    return run_recompute_fused(p, a, q, qd, workspace, stream);
+}
+
+int dfx_step_backward_mapped_recompute(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                                       const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                                       float* workspace, const float* gq_out, const float* gqd_out, const float* g_used,
+                                       float* gq, float* gqd, float* g_raw, void* stream) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !map || !raw) return (int)cudaErrorInvalidValue;
+    StepArgs a;
+    memset(&a, 0, sizeof a);
+    if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
+    if (!a.map_muscle && p->header.M > 0 && !act_other) return (int)cudaErrorInvalidValue;
+    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
+    a.dt_sub = (float)(dt / (double)substeps);
+    if (!recompute_fuses(p)) {
+        float* q_end = workspace_q_end(p, a, workspace);
+        const int e = dfx_step_forward_mapped(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end,
+                                              q_end + (long long)n * p->header.Q, workspace, stream);
+        if (e != 0) return e;
+        return dfx_step_backward_mapped(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, gq_out, gqd_out, g_used, gq, gqd, g_raw, stream);
+    }
+    a.raw = raw; a.gq_out = gq_out; a.gqd_out = gqd_out; a.g_used = g_used;
+    a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
+    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
+    return run_recompute_fused(p, a, q, qd, workspace, stream);
+}
+
+int dfx_env_step_backward_recompute(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                                    const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                                    float* workspace, const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !map || !raw || !tr) return (int)cudaErrorInvalidValue;
+    if (!transition_ok(tr->kind, tr->walker, tr->planar, p, map)) return (int)cudaErrorInvalidValue;
+    if (!tr->q_sim || !tr->qd_sim || !tr->used || !tr->reset || !tr->gq_sim || !tr->gqd_sim || !tr->g_used) return (int)cudaErrorInvalidValue;
+    StepArgs a;
+    memset(&a, 0, sizeof a);
+    if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
+    if (!a.map_muscle && p->header.M > 0 && !act_other) return (int)cudaErrorInvalidValue;
+    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
+    a.dt_sub = (float)(dt / (double)substeps);
+    if (!recompute_fuses(p) || !transition_fits(p, tr->kind, tr->walker, tr->planar, true)) {
+        // the plain mapped forward (the transition's outputs are not needed again: its adjoint reads tr->q_sim, ...), then the
+        // stored-tape entry, which runs the transition adjoint as its prologue or as a launch of its own
+        float* q_end = workspace_q_end(p, a, workspace);
+        const int e = dfx_step_forward_mapped(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end,
+                                              q_end + (long long)n * p->header.Q, workspace, stream);
+        if (e != 0) return e;
+        return dfx_env_step_backward(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, tr, gq, gqd, g_raw, stream);
+    }
+    a.raw = raw; a.gq_out = tr->gq_sim; a.gqd_out = tr->gqd_sim; a.g_used = tr->g_used;
+    a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
+    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
+    a.env_kind = tr->kind;
+    a.env_adj = *tr;
+    return run_recompute_fused(p, a, q, qd, workspace, stream);
+}
+
 }  // extern "C"

@@ -73,7 +73,8 @@ struct KernelArgs {
 #define DFX_DECLARE_TILE(E)                                                                                           \
     int dfx_tile_mode_e##E(int L, int D, int Q, int C, int M);      /* layout mode, or -1: no kernel of this width */  \
     size_t dfx_tile_smem_e##E(const void* kernel_args, int backward); /* dynamic shared memory (bytes) */             \
-    int dfx_tile_launch_e##E(void* kernel_args, int backward, void* stream);
+    int dfx_tile_launch_e##E(void* kernel_args, int backward, void* stream);                                         \
+    int dfx_tile_launch_recompute_e##E(void* kernel_args, void* stream);   /* forward into the workspace + adjoint, one launch */
 DFX_DECLARE_TILE(8)
 DFX_DECLARE_TILE(16)
 DFX_DECLARE_TILE(32)

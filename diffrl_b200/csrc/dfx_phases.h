@@ -657,9 +657,7 @@ DFX_HD void body_force_fwd(const Pack& P, const Layout& Y, SP s, const Grp& g) {
 }
 
 // adjoint: af[i] (adjoint of body_f_s[i]) plus what crba_adj left in aR[i] / au[i] -> aXsm, av, aa
-// ATOMIC_AV: another phase (the contact adjoint) adds to av concurrently
-template <bool ATOMIC_AV, class Grp>
-DFX_HD void body_force_link_adj(const Pack& P, const Layout& Y, SP s, int i, const Grp& g) {
+DFX_HD void body_force_link_adj(const Pack& P, const Layout& Y, SP s, int i) {
     const SP Xsm7 = s + Y.Xsm + i * 7;
     const BodyInertia B = body_inertia(P, Xsm7, i);
     const V3 c = ld3(Xsm7);
@@ -682,20 +680,14 @@ DFX_HD void body_force_link_adj(const Pack& P, const Layout& Y, SP s, int i, con
     outer_acc(aR, c, au);
     add3(s + Y.aXsm + i * 7, ac);
     add4(s + Y.aXsm + i * 7 + 3, q_to_m3_adj(ld4(Xsm7 + 3), aR));
-    if (ATOMIC_AV) {
-        const SP d = s + Y.av + i * 6;
-        g.atomic_add(&d[0], av.w.x); g.atomic_add(&d[1], av.w.y); g.atomic_add(&d[2], av.w.z);
-        g.atomic_add(&d[3], av.v.x); g.atomic_add(&d[4], av.v.y); g.atomic_add(&d[5], av.v.z);
-    } else {
-        add6(s + Y.av + i * 6, av);
-    }
+    add6(s + Y.av + i * 6, av);
     add6(s + Y.aa + i * 6, aa);
     kin_adj_local(P, Y, s, i);      // A1 of the kinematics adjoint, same link
 }
 
 template <class Grp>
 DFX_HD void body_force_adj(const Pack& P, const Layout& Y, SP s, const Grp& g) {
-    DFX_FOR(i, P.L) body_force_link_adj<false>(P, Y, s, i, g);
+    DFX_FOR(i, P.L) body_force_link_adj(P, Y, s, i);
     g.sync();
 }
 
@@ -852,9 +844,9 @@ DFX_HD void wrench_collect(const Pack& P, const Layout& Y, SP s, const Grp& g) {
     if (g.lane == 0) *poison = 0u;
 }
 
-// adjoint for one contact: cotangent r = af[body]; accumulates into aXsc[body], av[body] with shared-memory
-// atomics (only penetrating contacts do any work; the summation order, hence the last bits of the
-// GRADIENT, may vary between runs -- the forward pass stays deterministic)
+// adjoint for one contact: cotangent r = af[body]; accumulates into aXsc[body], av[body] (only penetrating contacts do
+// any work): muscle models through the fixed-point scatter, contact-only models with plain adds by the body's owner.
+// Either way the sums do not depend on thread timing, so the gradient is as bit-reproducible as the forward pass.
 template <class Grp>
 DFX_HD void contact_point_adj(const Pack& P, const Layout& Y, SP s, int k, float scale, const Grp& g) {
     const int b = P.cbody[k];
@@ -920,14 +912,14 @@ DFX_HD void contact_point_adj(const Pack& P, const Layout& Y, SP s, int k, float
         fx_scatter(sp_int(s + Y.aXsc) + b * 7, hi + b * 7, poison, b, c7, scale, g);
         fx_scatter(sp_int(s + Y.av) + b * 6, hi + P.L * 7 + b * 6, poison, b, c6, scale, g);
     } else {
-        // contact-only models: at most a handful of penetrating points share a body, and the compare-and-swap
-        // float add is then cheaper for the whole adjoint than fixed point + read-back (Ant and Humanoid).  The order of these few adds is not fixed, so the last bits of the gradient may vary.
+        // contact-only models: called by the item that owns body b (substep_adj), in the pack's contact order --
+        // one writer, a fixed order: plain adds, and the gradient is bit-reproducible
         const SP ax = s + Y.aXsc + b * 7;
         const SP avp = s + Y.av + b * 6;
 #pragma unroll
-        for (int c = 0; c < 7; ++c) g.atomic_add(&ax[c], c7[c]);
+        for (int c = 0; c < 7; ++c) ax[c] += c7[c];
 #pragma unroll
-        for (int c = 0; c < 6; ++c) g.atomic_add(&avp[c], c6[c]);
+        for (int c = 0; c < 6; ++c) avp[c] += c6[c];
     }
 }
 
@@ -1711,15 +1703,17 @@ DFX_HD void substep_adj(const Pack& P, const Layout& Y, SP s, float dt, bool app
         contact_adj(P, Y, s, g);
         adj_collect(P, Y, s, scale, g);
         body_force_adj(P, Y, s, g);
-    } else if (P.ground && Grp::kConcurrentItems) {
-        // contact-only model, CTA-wide barriers: the contact cotangents (compacted tasks, float atomics into aXsc / av)
-        // and the rigid-body force adjoint (one item per link, its av contribution by atomics too) as one phase
-        g.cta_compact_with(s, P.C, [&](SP se, int k) { return contact_penetrates(P, Y, se, k); },
-                           [&](SP se, int k) { contact_point_adj(P, Y, se, k, 1.0f, g); },
-                           P.L, [&](SP se, int i) { body_force_link_adj<true>(P, Y, se, i, g); });
     } else {
-        if (P.ground) contact_adj(P, Y, s, g);
-        body_force_adj(P, Y, s, g);
+        // contact-only model: one item per link -- its rigid-body force adjoint, then the cotangents of its own contact points
+        // in the pack's order (contacts are grouped by body, cbody_start).  Every av / aXsc entry has one writer adding in a
+        // fixed order, so the sums are bit-reproducible; float atomics from compacted contact tasks would add in an order that
+        // varies from run to run.  (A1 inside body_force_link_adj does not read what the contacts add.)
+        DFX_FOR(i, P.L) {
+            body_force_link_adj(P, Y, s, i);
+            if (P.ground)
+                for (int k = P.cbody_start[i]; k < P.cbody_start[i + 1]; ++k) contact_point_adj(P, Y, s, k, 1.0f, g);
+        }
+        g.sync();
     }
     g.phase_sync();
     kin_adj(P, Y, s, g);

@@ -61,6 +61,10 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 // make this thread's generic-proxy writes to shared memory visible to the async proxy (before a bulk store reads them)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// every bulk store of this thread has WRITTEN its destination (not only read its source, as bulk_wait_read_all)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// order async-proxy writes to global memory before this thread's later generic-proxy accesses
+__device__ __forceinline__ void fence_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 template <int NW, int E, bool PATH>
 struct GroupTile {
@@ -316,6 +320,71 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_kernel(const __grid_co
     g.finish();
 }
 
+// Recompute adjoint (include/dfx.h dfx_*_backward_recompute): the env-step's forward, re-run from its input state, writes the
+// tape of this tile into a caller-supplied one-env-step workspace (ka.step.tape, the tape's own layout) and the end state to
+// ka.step.q_out / qd_out (its tail); then the adjoint of dfx_tile_kernel<BACKWARD = true> reads that tape back
+// (ka.step.tape_in == ka.step.tape).  The forward is deterministic -- fixed-point scatter-adds, no float atomics -- so the
+// recomputed rows and H^-1 blocks are the stored tape's bit for bit.  Same set-up as dfx_tile_kernel (which stays as it is),
+// scratch sized for the larger of the two layouts, the backward's warps and occupancy.
+template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_recompute_kernel(const __grid_constant__ KernelArgs ka) {
+    constexpr int E = DFX_TILE_E;
+    extern __shared__ __align__(128) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += NW * 32) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += NW * 32) ipack[i] = ka.blob.ints[i];
+    int* cta_area = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    if (threadIdx.x < 4) cta_area[threadIdx.x] = 0;
+    unsigned long long* mbar = reinterpret_cast<unsigned long long*>(cta_area + 4);
+    if (threadIdx.x == 0) {
+        mbar_init(&mbar[0], 1);
+        mbar_init(&mbar[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+    P.jmask = tile_joint_mask(SL, SD, SQ, SC, SM);
+    constexpr Layout YF = make_layout(SL, SD, SQ, SC, SM, MODE, false);
+    constexpr Layout YB = make_layout(SL, SD, SQ, SC, SM, MODE, true);
+
+    GroupTile<NW, E, PATH> g;
+    const int lane32 = threadIdx.x & 31;
+    g.lane = (threadIdx.x >> 5) * (32 / E) + lane32 / E;
+    g.e = lane32 % E;
+    g.tile = blockIdx.x;
+    g.ntiles = gridDim.x;
+    g.task_count = cta_area;
+    g.task_list = cta_area + 8;
+    g.mbar = mbar;
+    g.par0 = g.par1 = 0u;
+    g.tile_base = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    int env = blockIdx.x * E + g.e;
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const SP s{g.tile_base + g.e};
+
+    env_step_forward(P, YF, s, g, env, ka.step);     // (no `used`, no derived dumps, no transition epilogue)
+    // The adjoint below reads the workspace the forward's bulk stores are still writing: TMA bulk loads of the rows (issued by
+    // thread 0) and, in the layouts without a staged H^-1 (Y.A < 0: the humanoids), plain loads of H^-1 rows by every thread.
+    //  1. every thread: fence its generic writes to the scratch tile against the async proxy -- the adjoint's bulk loads
+    //     overwrite the same bytes;
+    //  2. thread 0, the only issuer of bulk stores: wait_group 0 waits until they have WRITTEN global memory (wait_group.read,
+    //     all the forward needs, only waits until they have read the scratch), then a proxy fence orders those async-proxy
+    //     writes before generic-proxy accesses;
+    //  3. the CTA barrier publishes 1. and 2. to every thread: a bulk load issued or a plain load executed after it sees the
+    //     tape rows and H^-1 blocks the forward wrote.  Each CTA reads only its own tile's slots, so no other CTA is involved.
+    fence_async_smem();
+    if (threadIdx.x == 0) {
+        bulk_wait_all();
+        fence_async_global();
+    }
+    __syncthreads();
+    if (ka.step.env_kind) tile_transition_backward<NW * 32, E>(ka.step.env_kind, ka.step.env_adj, g.tile_base, ka.step.N);
+    env_step_backward(P, YB, s, g, env, ka.step);
+    g.finish();
+}
+
 // 128-byte aligned offsets so that the bulk copies of the tile stay 16-byte aligned
 static int tile_pack_floats(const KernelArgs& ka) {
     const int bytes = (((ka.blob.n_floats + 3) & ~3) + ((ka.blob.n_ints + 3) & ~3)) * 4;
@@ -335,6 +404,24 @@ static cudaError_t tile_launch_impl(KernelArgs& ka, cudaStream_t stream) {
     const size_t smem = (size_t)(ka.pack_smem_floats + ka.cta_area_floats + per_env * DFX_TILE_E) * sizeof(float);
     auto kern = dfx_tile_kernel<NW, MINB, BWD, PATH, MODE, SL, SD, SQ, SC, SM>;
     // (the opt-in to > 48 KB of dynamic shared memory is per device: set it on every launch, it is cheap)
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int ntiles = (ka.step.N + DFX_TILE_E - 1) / DFX_TILE_E;
+    kern<<<ntiles, NW * 32, smem, stream>>>(ka);
+    return cudaGetLastError();
+}
+
+template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+static cudaError_t tile_recompute_launch_impl(KernelArgs& ka, cudaStream_t stream) {
+    constexpr Layout YF = make_layout(SL, SD, SQ, SC, SM, MODE, false);
+    constexpr Layout YB = make_layout(SL, SD, SQ, SC, SM, MODE, true);
+    const int per_env = ((YF.fwd_size > YB.bwd_size ? YF.fwd_size : YB.bwd_size) + 3) & ~3;
+    ka.layout = YB;
+    ka.pack_smem_floats = tile_pack_floats(ka);
+    ka.cta_area_floats = tile_area_floats(ka);
+    ka.scratch_stride = per_env;
+    const size_t smem = (size_t)(ka.pack_smem_floats + ka.cta_area_floats + per_env * DFX_TILE_E) * sizeof(float);
+    auto kern = dfx_tile_recompute_kernel<NW, MINB, PATH, MODE, SL, SD, SQ, SC, SM>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     const int ntiles = (ka.step.N + DFX_TILE_E - 1) / DFX_TILE_E;
@@ -416,6 +503,21 @@ int DFX_TILE_FN(dfx_tile_launch)(void* kargs, int backward, void* stream) {
         return (int)(backward ? tile_launch_impl<nwb, minb, true, path, (mode) & 3, l, d, q, c, m>(ka, st)   \
                               : tile_launch_impl<nwf, minb, false, path, (mode) & 3, l, d, q, c, m>(ka, st));
     if (ka.step.flags & 64) { DFX_TILE_MODELS_ALT(X) }
+    DFX_TILE_MODELS(X)
+#undef X
+    return (int)cudaErrorInvalidConfiguration;
+}
+
+// the recompute adjoint (dfx_tile_recompute_kernel) of every DFX_TILE_MODELS entry, with the backward kernel's warps and
+// occupancy (every entry has as many forward as backward warps; tuning builds that set them apart run the forward part with
+// the backward's).  No flag-64 (A/B) variants: the caller runs the forward and the backward launches instead.
+int DFX_TILE_FN(dfx_tile_launch_recompute)(void* kargs, void* stream) {
+    KernelArgs& ka = *static_cast<KernelArgs*>(kargs);
+    const Pack& h = ka.header;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+#define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
+    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
+        return (int)tile_recompute_launch_impl<nwb, minb, path, (mode) & 3, l, d, q, c, m>(ka, st);
     DFX_TILE_MODELS(X)
 #undef X
     return (int)cudaErrorInvalidConfiguration;

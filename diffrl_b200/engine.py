@@ -7,7 +7,9 @@ every State tensor of every substep alive, forward writes one tape ROW per subst
 the forward intermediates the adjoint needs (X_sc, X_sm, S, v, a, total link wrenches, q'') -- and one H^-1 block
 per mass-matrix update; backward is one kernel that streams those rows back (TMA bulk copies in the tile
 kernels) and does NOT re-run the forward dynamics.  The tape is an opaque fp32 tensor sized by
-``dfx_tape_floats`` (optionally with bf16 (v, a, f_tot): ``diffrl_b200.set_tape_dtype``).
+``dfx_tape_floats`` (optionally with bf16 (v, a, f_tot): ``diffrl_b200.set_tape_dtype``).  In recompute mode
+(``diffrl_b200.set_adjoint_mode("recompute")``) the forward keeps no tape: the backward re-runs the env-step's forward
+into a one-env-step workspace inside its adjoint launch.
 """
 import ctypes
 
@@ -21,6 +23,14 @@ _DERIVED_SHAPES = {
     "body_a_s": ("L", 6), "body_f_s": ("L", 6), "body_ft_s": ("L", 6), "joint_tau": ("D", 0),
     "joint_qdd": ("D", 0), "H": ("DD", 0), "L": ("DD", 0),
 }
+
+
+ADJOINT_MODES = ("tape", "recompute")
+adjoint_mode = "tape"        # diffrl_b200.set_adjoint_mode; the step ops read it in forward and keep it on ctx
+
+
+def recompute_adjoint():
+    return adjoint_mode == "recompute"
 
 
 def _ptr(t):
@@ -112,8 +122,27 @@ class ArticulationEngine:
             t = torch.cat([lo, halves, t[:, :, head + mid // 2:]], dim=2)
         return t.permute(0, 1, 3, 2).reshape(substeps, ntiles * tile, row)[:, : self.N].contiguous()
 
+    def tape_hinv(self, tape, substeps, mm_freq):
+        """The H^-1 blocks of the tape (every mass-matrix update, every environment slot of the kernel family's layout) as a
+        NEW flat tensor (tests)."""
+        tile = int(self.lib.dfx_pack_query(self.pack, 9))
+        slots = (self.N + tile - 1) // tile * tile if tile else self.N
+        end = self.tape_floats(substeps, mm_freq)
+        nseg = (substeps + mm_freq - 1) // mm_freq
+        return tape[end - nseg * slots * self.D * self.D:end].clone()
+
     def tape_floats(self, substeps, mm_freq):
         return int(self.lib.dfx_tape_floats(self.pack, self.N, substeps, mm_freq))
+
+    def recompute_workspace(self, substeps, mm_freq):
+        """An uninitialised workspace for one recompute adjoint: one env-step's tape + its end state (include/dfx.h)."""
+        n = int(self.lib.dfx_recompute_workspace_floats(self.pack, self.N, int(substeps), int(mm_freq)))
+        return torch.empty(n, dtype=torch.float32, device=self.device)
+
+    def workspace_end_state(self, workspace, substeps, mm_freq):
+        """(q_out, qd_out) of the forward a recompute adjoint re-ran into ``workspace`` (views)."""
+        t, nq = self.tape_floats(substeps, mm_freq), self.N * self.Q
+        return workspace[t:t + nq], workspace[t + nq:t + nq + self.N * self.D]
 
     def _stream(self):
         return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
@@ -171,6 +200,30 @@ class ArticulationEngine:
         _capi.check(code, "dfx_step_backward")
         return gq, gqd, gact, gmusc
 
+    def backward_recompute(self, q, qd, act, musc, gq_out, gqd_out, substeps, mm_freq, dt, need=(True, True, True, True),
+                           workspace=None):
+        """``backward`` without a tape: the env-step's forward from (q, qd, act, musc) is re-run into a workspace inside the
+        adjoint launch (``dfx_step_backward_recompute``).  ``workspace`` (``recompute_workspace()``): used and left readable
+        (``tape_rows``, ``tape_hinv``, ``workspace_end_state``); None: one from the caching allocator."""
+        dev = self.device
+        q, qd, act = _f32c(q, dev), _f32c(qd, dev), _f32c(act, dev)
+        musc = _f32c(musc, dev) if self.M else None
+        gq_out = None if gq_out is None else _f32c(gq_out, dev)
+        gqd_out = None if gqd_out is None else _f32c(gqd_out, dev)
+        if workspace is None:
+            workspace = self.recompute_workspace(substeps, mm_freq)
+        gq = torch.empty(self.N * self.Q, dtype=torch.float32, device=dev) if need[0] else None
+        gqd = torch.empty(self.N * self.D, dtype=torch.float32, device=dev) if need[1] else None
+        gact = torch.empty(self.N * self.D, dtype=torch.float32, device=dev) if need[2] else None
+        gmusc = torch.empty(self.N * self.M, dtype=torch.float32, device=dev) if (need[3] and self.M) else None
+        with torch.cuda.device(dev):
+            code = self.lib.dfx_step_backward_recompute(self.pack, self.N, int(substeps), int(mm_freq), float(dt),
+                                                        _ptr(q), _ptr(qd), _ptr(act), _ptr(musc), _ptr(workspace),
+                                                        _ptr(gq_out), _ptr(gqd_out), _ptr(gq), _ptr(gqd), _ptr(gact), _ptr(gmusc),
+                                                        self._stream())
+        _capi.check(code, "dfx_step_backward_recompute")
+        return gq, gqd, gact, gmusc
+
 
 class MappedSimStepFunction(torch.autograd.Function):
     """(q, qd, raw policy output) -> (q', qd', used): the env-step with the action map folded into the simulation launch
@@ -188,8 +241,9 @@ class MappedSimStepFunction(torch.autograd.Function):
         n, A = engine.N, raw.shape[-1]
         m = DfxActionMap(int(A), int(offset), int(bool(is_muscle)), float(pre_scale), float(pre_bias), float(drive_scale), strength.data_ptr())
         need = any(ctx.needs_input_grad[5:8])
+        ctx.recompute = recompute_adjoint()
         q_out, qd_out, used = torch.empty_like(q), torch.empty_like(qd), torch.empty_like(raw)
-        tape = torch.empty(engine.tape_floats(substeps, mm_freq), dtype=torch.float32, device=dev) if need else None
+        tape = torch.empty(engine.tape_floats(substeps, mm_freq), dtype=torch.float32, device=dev) if (need and not ctx.recompute) else None
         with torch.cuda.device(dev):
             code = engine.lib.dfx_step_forward_mapped(engine.pack, n, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd),
                                                       ctypes.byref(m), _ptr(raw), None, _ptr(used), _ptr(q_out), _ptr(qd_out),
@@ -199,12 +253,14 @@ class MappedSimStepFunction(torch.autograd.Function):
         ctx.strength = strength                      # keeps the device array the struct points at alive
         ctx.set_materialize_grads(False)
         ctx.shapes = (q.shape, qd.shape)
-        ctx.save_for_backward(raw, tape)
+        if ctx.recompute:
+            ctx.save_for_backward(raw, q, qd)        # the env-step's input state, in place of its tape
+        else:
+            ctx.save_for_backward(raw, tape)
         return q_out, qd_out, used
 
     @staticmethod
     def backward(ctx, gq_out, gqd_out, g_used):
-        raw, tape = ctx.saved_tensors
         engine, (substeps, mm_freq, dt) = ctx.engine, ctx.cfg
         dev = engine.device
         gq_out = None if gq_out is None else _f32c(gq_out, dev)
@@ -212,12 +268,23 @@ class MappedSimStepFunction(torch.autograd.Function):
         g_used = None if g_used is None else _f32c(g_used, dev)
         gq = torch.empty(engine.N * engine.Q, dtype=torch.float32, device=dev)
         gqd = torch.empty(engine.N * engine.D, dtype=torch.float32, device=dev)
-        g_raw = torch.empty_like(raw)
-        with torch.cuda.device(dev):
-            code = engine.lib.dfx_step_backward_mapped(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), ctypes.byref(ctx.amap),
-                                                       _ptr(raw), None, _ptr(tape), _ptr(gq_out), _ptr(gqd_out), _ptr(g_used),
-                                                       _ptr(gq), _ptr(gqd), _ptr(g_raw), engine._stream())
-        _capi.check(code, "dfx_step_backward_mapped")
+        cot = (_ptr(gq_out), _ptr(gqd_out), _ptr(g_used), _ptr(gq), _ptr(gqd))
+        if ctx.recompute:
+            raw, q, qd = ctx.saved_tensors
+            g_raw = torch.empty_like(raw)
+            workspace = engine.recompute_workspace(substeps, mm_freq)
+            with torch.cuda.device(dev):
+                code = engine.lib.dfx_step_backward_mapped_recompute(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt),
+                                                                     _ptr(q), _ptr(qd), ctypes.byref(ctx.amap), _ptr(raw), None,
+                                                                     _ptr(workspace), *cot, _ptr(g_raw), engine._stream())
+            _capi.check(code, "dfx_step_backward_mapped_recompute")
+        else:
+            raw, tape = ctx.saved_tensors
+            g_raw = torch.empty_like(raw)
+            with torch.cuda.device(dev):
+                code = engine.lib.dfx_step_backward_mapped(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), ctypes.byref(ctx.amap),
+                                                           _ptr(raw), None, _ptr(tape), *cot, _ptr(g_raw), engine._stream())
+            _capi.check(code, "dfx_step_backward_mapped")
         return None, None, None, None, None, gq.view(ctx.shapes[0]), gqd.view(ctx.shapes[1]), g_raw
 
 
@@ -227,21 +294,31 @@ class SimStepFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, engine, substeps, mm_freq, dt, q, qd, act, musc):
         needs = ctx.needs_input_grad[4:8]
+        ctx.recompute = recompute_adjoint()
         q_out, qd_out, tape, _ = engine.forward(q.detach(), qd.detach(), act.detach(),
                                                 None if musc is None else musc.detach(),
-                                                substeps, mm_freq, dt, want_tape=any(needs))
+                                                substeps, mm_freq, dt, want_tape=any(needs) and not ctx.recompute)
         ctx.engine, ctx.cfg, ctx.needs = engine, (substeps, mm_freq, dt), needs
         ctx.set_materialize_grads(False)      # a missing cotangent is NULL for dfx_step_backward, not a zero fill
         ctx.shapes = (q.shape, qd.shape, act.shape, None if musc is None else musc.shape)
-        ctx.save_for_backward(act.detach(), musc.detach() if (musc is not None and engine.M) else None, tape)
+        musc = musc.detach() if (musc is not None and engine.M) else None
+        if ctx.recompute:
+            ctx.save_for_backward(act.detach(), musc, q.detach(), qd.detach())   # the env-step's input state, in place of its tape
+        else:
+            ctx.save_for_backward(act.detach(), musc, tape)
         return q_out.view(q.shape), qd_out.view(qd.shape)
 
     @staticmethod
     def backward(ctx, gq_out, gqd_out):
-        act, musc, tape = ctx.saved_tensors
         substeps, mm_freq, dt = ctx.cfg
-        gq, gqd, gact, gmusc = ctx.engine.backward(act, musc, tape, gq_out, gqd_out, substeps, mm_freq, dt,
-                                                   need=tuple(ctx.needs))
+        if ctx.recompute:
+            act, musc, q, qd = ctx.saved_tensors
+            gq, gqd, gact, gmusc = ctx.engine.backward_recompute(q, qd, act, musc, gq_out, gqd_out, substeps, mm_freq, dt,
+                                                                 need=tuple(ctx.needs))
+        else:
+            act, musc, tape = ctx.saved_tensors
+            gq, gqd, gact, gmusc = ctx.engine.backward(act, musc, tape, gq_out, gqd_out, substeps, mm_freq, dt,
+                                                       need=tuple(ctx.needs))
         sq, sqd, sact, smusc = ctx.shapes
         return (None, None, None, None,
                 None if gq is None else gq.view(sq), None if gqd is None else gqd.view(sqd),

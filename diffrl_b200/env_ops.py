@@ -5,6 +5,7 @@ import ctypes
 import torch
 
 from . import _capi
+from .engine import recompute_adjoint
 
 
 class DfxWalkerParams(ctypes.Structure):
@@ -70,6 +71,8 @@ def _bind(lib):
     Dbl = ctypes.c_double
     lib.dfx_env_step_forward.argtypes = [V, I, I, I, Dbl, V, V, V, V, V, V, V, V, V, ctypes.POINTER(DfxEnvTransition), V]
     lib.dfx_env_step_backward.argtypes = [V, I, I, I, Dbl, V, V, V, V, ctypes.POINTER(DfxEnvTransitionAdj), V, V, V, V]
+    if hasattr(lib, "dfx_env_step_backward_recompute"):
+        lib.dfx_env_step_backward_recompute.argtypes = [V, I, I, I, Dbl, V, V, V, V, V, V, ctypes.POINTER(DfxEnvTransitionAdj), V, V, V, V]
     lib._walker_bound = True
 
 
@@ -245,7 +248,8 @@ class EnvStepFunction(torch.autograd.Function):
         q_sim, qd_sim, used = torch.empty_like(q), torch.empty_like(qd), torch.empty_like(raw)
         need = any(ctx.needs_input_grad[10:13])
         ctx.nan_guard = nan_guard
-        tape = torch.empty(engine.tape_floats(substeps, mm_freq), **f32) if need else None
+        ctx.recompute = recompute_adjoint()
+        tape = torch.empty(engine.tape_floats(substeps, mm_freq), **f32) if (need and not ctx.recompute) else None
         obs_before = torch.empty((n, params.num_obs), **f32)
         obs_next = torch.empty((n, params.num_obs), **f32)
         rew = torch.empty(n, **f32)
@@ -270,13 +274,14 @@ class EnvStepFunction(torch.autograd.Function):
         ctx.strength = strength                      # keeps the device array the struct points at alive
         ctx.set_materialize_grads(False)             # absent cotangents arrive as None (NULL in the C ABI), not as zero fills
         ctx.shapes = (q.shape, qd.shape)
-        ctx.save_for_backward(raw, tape, q_sim, qd_sim, used, reset)
+        # recompute mode: the env-step's input state in place of its tape
+        ctx.save_for_backward(raw, tape, q_sim, qd_sim, used, reset, *((q, qd) if ctx.recompute else (None, None)))
         ctx.mark_non_differentiable(reset, progress_next)
         return obs_before, rew, reset, q_next, qd_next, actions_next, progress_next, obs_next
 
     @staticmethod
     def backward(ctx, g_obs_before, g_rew, g_reset, g_q_next, g_qd_next, g_actions_next, g_progress, g_obs_next):
-        raw, tape, q_sim, qd_sim, used, reset = ctx.saved_tensors
+        raw, tape, q_sim, qd_sim, used, reset, q, qd = ctx.saved_tensors
         engine, (substeps, mm_freq, dt), params = ctx.engine, ctx.cfg, ctx.params
         lib, dev = engine.lib, engine.device
         cot = [None if g is None else _c(g) for g in (g_obs_before, g_rew, g_q_next, g_qd_next, g_actions_next, g_obs_next)]
@@ -295,10 +300,18 @@ class EnvStepFunction(torch.autograd.Function):
         gq = torch.empty(engine.N * engine.Q, dtype=torch.float32, device=dev)
         gqd = torch.empty(engine.N * engine.D, dtype=torch.float32, device=dev)
         g_raw = torch.empty_like(raw)
-        with torch.cuda.device(dev):
-            code = lib.dfx_env_step_backward(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), ctypes.byref(ctx.amap), _ptr(raw),
-                                             None, _ptr(tape), ctypes.byref(tr), _ptr(gq), _ptr(gqd), _ptr(g_raw), _stream(dev))
-        _capi.check(code, "dfx_env_step_backward")
+        if ctx.recompute:
+            workspace = engine.recompute_workspace(substeps, mm_freq)
+            with torch.cuda.device(dev):
+                code = lib.dfx_env_step_backward_recompute(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd),
+                                                           ctypes.byref(ctx.amap), _ptr(raw), None, _ptr(workspace), ctypes.byref(tr),
+                                                           _ptr(gq), _ptr(gqd), _ptr(g_raw), _stream(dev))
+            _capi.check(code, "dfx_env_step_backward_recompute")
+        else:
+            with torch.cuda.device(dev):
+                code = lib.dfx_env_step_backward(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), ctypes.byref(ctx.amap), _ptr(raw),
+                                                 None, _ptr(tape), ctypes.byref(tr), _ptr(gq), _ptr(gqd), _ptr(g_raw), _stream(dev))
+            _capi.check(code, "dfx_env_step_backward")
         if ctx.nan_guard:
             for g in (gq, gqd, g_raw):
                 torch.nan_to_num(g, nan=0.0, posinf=0.0, neginf=0.0, out=g)

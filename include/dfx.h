@@ -289,6 +289,34 @@ int dfx_env_step_backward(const dfx_pack_t* pack, int n, int substeps, int mm_fr
                           const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
                           const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream);
 
+/* ---- recompute adjoint: backward WITHOUT a stored tape.  The forward then runs with tape == NULL (the no-grad launch) and
+ * keeps nothing; each adjoint entry below re-runs the env-step's forward from its input state (q, qd) and actuation into a
+ * workspace that holds ONE env-step's tape, then runs the adjoint of its stored-tape twin on it.  The forward is deterministic
+ * (fixed-point scatter-adds), so the recomputed tape is the stored tape bit for bit and so are the cotangents: memory
+ * O(one env-step) instead of O(horizon), for one extra forward per env-step in the backward.
+ *
+ * Workspace: dfx_recompute_workspace_floats(pack, n, substeps, mm_freq) floats, device memory, contents on entry ignored.  On
+ * return it holds the recomputed tape in the tape's layout at offset 0 (dfx_tape_floats(pack, n, substeps, mm_freq) floats),
+ * then the end state of the recomputed forward: q_out [n*Q] at offset dfx_tape_floats(...), qd_out [n*D] right after it.
+ * It may be reused by the next call on the same stream.
+ *
+ * Tile kernels: ONE launch (the forward into the workspace and the adjoint in the same CTA).  Lane-group kernels, the A/B
+ * variants of dfx_set_flags bit 6 and env-steps whose transition adjoint cannot be staged in the tile: the forward launch, then
+ * the stored-tape entry on the workspace.  Arguments as the twin, with `tape` replaced by q [n*Q], qd [n*D] (the inputs of the
+ * forward call, not modified) and `workspace`; a NULL q, qd or workspace is cudaErrorInvalidValue. */
+long long dfx_recompute_workspace_floats(const dfx_pack_t* pack, int num_envs, int substeps, int mm_freq);
+int dfx_step_backward_recompute(const dfx_pack_t* pack, int num_envs, int substeps, int mm_freq, double dt,
+                                const float* q, const float* qd, const float* act, const float* musc, float* workspace,
+                                const float* gq_out, const float* gqd_out,
+                                float* gq, float* gqd, float* gact, float* gmusc, void* stream);
+int dfx_step_backward_mapped_recompute(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
+                                       const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                                       float* workspace, const float* gq_out, const float* gqd_out, const float* g_used,
+                                       float* gq, float* gqd, float* g_raw, void* stream);
+int dfx_env_step_backward_recompute(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
+                                    const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                                    float* workspace, const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream);
+
 /* Launch configuration knob: lanes cooperating on one environment (8, 16 or 32; 0 = auto). */
 int dfx_set_group_size(int lanes);
 /* Tuning flags (default 9; for A/B timing and tests).  Lane-group kernels: bit 1 (2) = extra CTA-wide barriers between
