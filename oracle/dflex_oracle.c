@@ -11,11 +11,15 @@
  * tests/test_oracle.py against the golden vectors recorded from the unmodified reference
  * (oracle/make_golden.py) and against the reference's own compiled kernels (oracle/ref_driver.py).
  *
- * Built twice (oracle/Makefile): REAL=float -> liboracle_f32.so (forward parity) and REAL=double ->
+ * Built three times (oracle/Makefile): REAL=float -> liboracle_f32.so (forward parity), REAL=double ->
  * liboracle_f64.so, whose central finite differences of sum(gq.q' + gqd.qd') check the hand-derived
- * adjoint kernels independently of any adjoint code (oracle_fd_gradient below).
+ * adjoint kernels independently of any adjoint code (oracle_fd_gradient below), and REAL=double _Complex ->
+ * liboracle_c64.so, whose complex-step derivative of the same loss is exact to rounding on the branches the
+ * fp64 forward takes (oracle_exact_gradient).  Every comparison of reals goes through RLT / RGT / RGE, so the
+ * three builds take their branches on the same (real) values; the f32 and f64 arithmetic is unchanged by it.
  */
 #include <math.h>
+#include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -25,9 +29,39 @@
 #define REAL float
 #endif
 typedef REAL real;
+#ifdef ORACLE_COMPLEX
+/* Complex-step build (REAL = double _Complex): every input carries an imaginary perturbation i*h, every branch is decided
+ * on the real part, so Im(output)/h is the exact derivative of the branch actually taken (oracle_exact_gradient). */
+#include <complex.h>
+#undef I   /* the inertia parameter below is named I */
+#define RE(x) creal(x)
+#define R_SQRT(x) csqrt(x)
+#define R_SIN(x) csin(x)
+#define R_COS(x) ccos(x)
+#else
+#define RE(x) (x)
 #define R_SQRT(x) ((real)sqrt((double)(x)))
 #define R_SIN(x) ((sizeof(real) == 4) ? (real)sinf((float)(x)) : (real)sin((double)(x)))
 #define R_COS(x) ((sizeof(real) == 4) ? (real)cosf((float)(x)) : (real)cos((double)(x)))
+#endif
+/* every comparison of reals goes through these: real parts in the complex build, the plain comparison otherwise */
+#define RLT(a, b) (RE(a) < RE(b))
+#define RGT(a, b) (RE(a) > RE(b))
+#define RGE(a, b) (RE(a) >= RE(b))
+
+/* Branch record (oracle_branch_signature): the decisions of the contact and joint-limit model, in the order they are taken */
+enum { BR_PENETRATE, BR_VN_NEG, BR_CAP_VISCOUS, BR_CAP_COULOMB, BR_LOWER, BR_UPPER, BR_COUNT };
+static struct { int on; uint64_t hash; int64_t counts[BR_COUNT]; } g_branch;
+static int branch_record(int kind, int taken) {
+    if (g_branch.on) {
+        /* FNV-1a over (kind, taken); the friction cap records which of its two branches was taken */
+        g_branch.hash = (g_branch.hash ^ (uint64_t)(2 * kind + (taken != 0))) * 1099511628211ull;
+        if (kind == BR_CAP_VISCOUS) g_branch.counts[taken ? BR_CAP_VISCOUS : BR_CAP_COULOMB]++;
+        else if (taken) g_branch.counts[kind]++;
+    }
+    return taken;
+}
+#define BRANCH(kind, cond) branch_record((kind), (cond))
 
 typedef struct { real x, y, z; } v3;
 typedef struct { real x, y, z, w; } q4;
@@ -44,7 +78,7 @@ static real vdot(v3 a, v3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
 static v3 vcross(v3 a, v3 b) { return V(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x); }
 static real vlen(v3 a) { return R_SQRT(vdot(a, a)); }
 /* vec3.h:96-103: zero vector for zero length (kEps = 0, adjoint.h:73) */
-static v3 vnormalize(v3 a) { real l = vlen(a); return l > 0 ? V(a.x / l, a.y / l, a.z / l) : V(0, 0, 0); }
+static v3 vnormalize(v3 a) { real l = vlen(a); return RGT(l, 0) ? V(a.x / l, a.y / l, a.z / l) : V(0, 0, 0); }
 
 /* ---- quat.h:44-116 */
 static q4 Qn(real x, real y, real z, real w) { q4 r = {x, y, z, w}; return r; }
@@ -64,7 +98,7 @@ static v3 rotate(q4 q, v3 x) { /* quat.h:113-116 */
 static q4 qinverse(q4 q) { return Qn(-q.x, -q.y, -q.z, q.w); }
 static q4 qnormalize(q4 q) { /* quat.h:70-83 */
     real l = R_SQRT(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
-    if (l > 0) { real inv = (real)1 / l; return Qn(q.x * inv, q.y * inv, q.z * inv, q.w * inv); }
+    if (RGT(l, 0)) { real inv = (real)1 / l; return Qn(q.x * inv, q.y * inv, q.z * inv, q.w * inv); }
     return Qn(0, 0, 0, 1);
 }
 
@@ -191,14 +225,14 @@ static void eval_rigid_contacts(const Art* a, Work* w) {
         v3 p = vsub(xf_point(w->X_sc[b], ld3(a->m->contact_point0 + k * 3)), vmul(n, (real)a->m->contact_dist[k]));
         v3 dpdt = vadd(w->v_s[b].v, vcross(w->v_s[b].w, p));
         real c = vdot(n, p);
-        if (c >= 0) continue;
+        if (BRANCH(BR_PENETRATE, RLT(c, 0)) == 0) continue;
         real vn = vdot(n, dpdt);
         v3 vt = vsub(dpdt, vmul(n, vn));
         real fn = c * ke;
-        real stepc = c < 0 ? (real)1 : (real)0;
-        real fd = (vn < 0 ? vn : (real)0) * kd * stepc * ((real)0 - c);
+        real stepc = RLT(c, 0) ? (real)1 : (real)0;
+        real fd = (BRANCH(BR_VN_NEG, RLT(vn, 0)) ? vn : (real)0) * kd * stepc * ((real)0 - c);
         real cap_a = kf * vlen(vt), cap_b = (real)0 - mu * c * ke;
-        v3 ft = vmul(vmul(vnormalize(vt), cap_a < cap_b ? cap_a : cap_b), stepc);
+        v3 ft = vmul(vmul(vnormalize(vt), (BRANCH(BR_CAP_VISCOUS, RLT(cap_a, cap_b)) ? cap_a : cap_b)), stepc);
         v3 f_total = vadd(vmul(n, fn + fd), ft);
         v3 t_total = vcross(p, f_total);
         w->f_s[b] = sv_add(w->f_s[b], SVn(t_total, f_total));
@@ -227,8 +261,8 @@ static void eval_rigid_tau(const Art* a, const real* q, const real* qd, const re
         sv f_s = sv_add(w->f_s[i], w->ft_s[i]);
         if (type == 0 || type == 1) {
             real qq = q[cs], qdv = qd[ds], lower = F(joint_limit_lower, cs), upper = F(joint_limit_upper, cs), limit_f = 0;
-            if (qq < lower) limit_f = lke * (lower - qq);
-            if (qq > upper) limit_f = lke * (upper - qq);
+            if (BRANCH(BR_LOWER, RLT(qq, lower))) limit_f = lke * (lower - qq);
+            if (BRANCH(BR_UPPER, RGT(qq, upper))) limit_f = lke * (upper - qq);
             real damping_f = ((real)0 - lkd) * qdv;
             w->tau[ds] = (real)0 - sv_dot(w->S_s[ds], f_s) - tke * (qq - F(joint_target, cs)) - tkd * qdv + act[ds] + limit_f + damping_f;
         }
@@ -367,9 +401,9 @@ void oracle_step_forward(const DfxModelDesc* m, int n, int substeps, int mm_freq
         for (int i = 0; i < D; ++i) { rqd[i] = (real)qd[(size_t)e * D + i]; ract[i] = (real)act[(size_t)e * D + i]; }
         for (int i = 0; i < M; ++i) rm[i] = (real)musc[(size_t)e * M + i];
         env_step_one(&a, &w, rq, rqd, ract, rm, dt, substeps, mm_freq, rt);
-        for (int i = 0; i < Q; ++i) q_out[(size_t)e * Q + i] = (double)rq[i];
-        for (int i = 0; i < D; ++i) qd_out[(size_t)e * D + i] = (double)rqd[i];
-        if (traj) for (size_t i = 0; i < (size_t)substeps * (Q + D); ++i) traj[(size_t)e * substeps * (Q + D) + i] = (double)rt[i];
+        for (int i = 0; i < Q; ++i) q_out[(size_t)e * Q + i] = (double)RE(rq[i]);
+        for (int i = 0; i < D; ++i) qd_out[(size_t)e * D + i] = (double)RE(rqd[i]);
+        if (traj) for (size_t i = 0; i < (size_t)substeps * (Q + D); ++i) traj[(size_t)e * substeps * (Q + D) + i] = (double)RE(rt[i]);
     }
     free(rq); free(rqd); free(ract); free(rm); free(rt);
     work_free(&w);
@@ -387,8 +421,8 @@ static double loss_of(const Art* a, Work* w, const double* q, const double* qd, 
     for (int i = 0; i < M; ++i) rm[i] = (real)musc[i];
     env_step_one(a, w, rq, rqd, ract, rm, dt, substeps, mm_freq, NULL);
     double loss = 0;
-    for (int i = 0; i < Q; ++i) loss += gq_out[i] * (double)rq[i];
-    for (int i = 0; i < D; ++i) loss += gqd_out[i] * (double)rqd[i];
+    for (int i = 0; i < Q; ++i) loss += gq_out[i] * (double)RE(rq[i]);
+    for (int i = 0; i < D; ++i) loss += gqd_out[i] * (double)RE(rqd[i]);
     free(rq); free(rqd); free(ract); free(rm);
     return loss;
 }
@@ -420,3 +454,64 @@ void oracle_fd_gradient(const DfxModelDesc* m, int substeps, int mm_freq, double
     }
     work_free(&w);
 }
+
+/* Per environment: a 64-bit FNV-1a hash of the sequence of branch decisions of the contact and joint-limit model over all
+ * substeps (contact penetrates, vn < 0, friction cap viscous / Coulomb, q < lower, q > upper) and the count of each
+ * (counts [n, BR_COUNT] in the order of the BR_ enum).  The f32 and f64 builds decide on their own rounding. */
+void oracle_branch_signature(const DfxModelDesc* m, int n, int substeps, int mm_freq, double dt,
+                             const double* q, const double* qd, const double* act, const double* musc,
+                             uint64_t* hash, int64_t* counts) {
+    int Q = m->coord_count, D = m->dof_count, M = m->muscle_count;
+    double* q_out = malloc(sizeof(double) * (Q + 1)); double* qd_out = malloc(sizeof(double) * (D + 1));
+    for (int e = 0; e < n; ++e) {
+        memset(&g_branch, 0, sizeof g_branch);
+        g_branch.on = 1; g_branch.hash = 14695981039346656037ull;
+        oracle_step_forward(m, 1, substeps, mm_freq, dt, q + (size_t)e * Q, qd + (size_t)e * D, act + (size_t)e * D,
+                            musc + (size_t)e * M, q_out, qd_out, NULL);
+        hash[e] = g_branch.hash;
+        for (int k = 0; k < BR_COUNT; ++k) counts[(size_t)e * BR_COUNT + k] = g_branch.counts[k];
+    }
+    g_branch.on = 0;
+    free(q_out); free(qd_out);
+}
+
+#ifdef ORACLE_COMPLEX
+/* Complex-step derivative of  loss = gq_out . q' + gqd_out . qd'  w.r.t. every input of ONE environment (same signature
+ * as oracle_fd_gradient; h is the imaginary step, 1e-30 when h <= 0).  One complex forward per input component:
+ * dloss/dx_i = Im loss(x + i h e_i) / h.  Nothing is subtracted, so the result is exact to rounding for the branch the
+ * real part takes -- the quantity a reverse-mode adjoint of the same forward computes. */
+void oracle_exact_gradient(const DfxModelDesc* m, int substeps, int mm_freq, double dt, double h,
+                           const double* q, const double* qd, const double* act, const double* musc,
+                           const double* gq_out, const double* gqd_out,
+                           double* gq, double* gqd, double* gact, double* gmusc) {
+    Art a = make_art(m);
+    Work w = work_alloc(&a);
+    int Q = a.Q, D = a.D, M = a.M;
+    int sizes[4] = {Q, D, D, M};
+    const double* base[4] = {q, qd, act, musc};
+    double* outs[4] = {gq, gqd, gact, gmusc};
+    real* in[4];
+    for (int g = 0; g < 4; ++g) {
+        in[g] = malloc(sizeof(real) * (sizes[g] + 1));
+        for (int i = 0; i < sizes[g]; ++i) in[g][i] = base[g][i];
+    }
+    real* rq = malloc(sizeof(real) * (Q + 1)); real* rqd = malloc(sizeof(real) * (D + 1));
+    if (!(h > 0)) h = 1e-30;
+    for (int g = 0; g < 4; ++g) {
+        if (!outs[g]) continue;
+        for (int i = 0; i < sizes[g]; ++i) {
+            in[g][i] = CMPLX(base[g][i], h);
+            memcpy(rq, in[0], sizeof(real) * Q); memcpy(rqd, in[1], sizeof(real) * D);
+            env_step_one(&a, &w, rq, rqd, in[2], in[3], dt, substeps, mm_freq, NULL);
+            double s = 0;
+            for (int k = 0; k < Q; ++k) s += gq_out[k] * cimag(rq[k]);
+            for (int k = 0; k < D; ++k) s += gqd_out[k] * cimag(rqd[k]);
+            outs[g][i] = s / h;
+            in[g][i] = base[g][i];
+        }
+    }
+    for (int g = 0; g < 4; ++g) free(in[g]);
+    free(rq); free(rqd);
+    work_free(&w);
+}
+#endif

@@ -12,6 +12,9 @@ from diffrl_b200.modelpack import DfxModelDesc, articulation_from_model  # noqa:
 
 _D = ctypes.POINTER(ctypes.c_double)
 _libs = {}
+# columns of Oracle.branches' counts (dflex_oracle.c BR_*): penetrating contact points, of those with vn < 0, friction capped
+# by kf |vt| (viscous) / by mu |fn| (Coulomb), joint coordinate below its lower / above its upper limit; summed over substeps
+BRANCHES = ("penetrate", "vn_neg", "cap_viscous", "cap_coulomb", "lower", "upper")
 
 
 def _lib(precision):
@@ -25,7 +28,11 @@ def _lib(precision):
                                             _D, _D, _D, _D, _D, _D, _D]
         lib.oracle_fd_gradient.argtypes = [ctypes.POINTER(DfxModelDesc), ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_double,
                                            _D, _D, _D, _D, _D, _D, _D, _D, _D, _D]
-        assert lib.oracle_real_bytes() == (4 if precision == "f32" else 8)
+        lib.oracle_branch_signature.argtypes = [ctypes.POINTER(DfxModelDesc), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
+                                                _D, _D, _D, _D, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_int64)]
+        if precision == "c64":
+            lib.oracle_exact_gradient.argtypes = lib.oracle_fd_gradient.argtypes
+        assert lib.oracle_real_bytes() == {"f32": 4, "f64": 8, "c64": 16}[precision]
         _libs[precision] = lib
     return _libs[precision]
 
@@ -57,6 +64,36 @@ class Oracle:
         _lib(precision).oracle_step_forward(ctypes.byref(self.struct), n, substeps, mm_freq, float(dt), _p(q), _p(qd), _p(act),
                                             _p(musc), _p(q_out), _p(qd_out), _p(traj))
         return (q_out, qd_out, traj) if want_traj else (q_out, qd_out)
+
+    def _inputs(self, q, qd, act, musc):
+        d = self.desc
+        f = lambda a: np.ascontiguousarray(a, np.float64).ravel()
+        q, qd, act = f(q), f(qd), f(act)
+        n = q.size // d.Q
+        musc = np.zeros(max(1, n * d.M)) if musc is None or d.M == 0 else f(musc)
+        return n, q, qd, act, musc
+
+    def branches(self, q, qd, act, musc, substeps, mm_freq, dt, precision="f64"):
+        """Per environment: (hash [n] uint64 of the sequence of contact / limit branch decisions over all substeps,
+        counts [n, 6] int64 in the order of BRANCHES), in the f32 or the f64 build."""
+        n, q, qd, act, musc = self._inputs(q, qd, act, musc)
+        h, c = np.zeros(n, np.uint64), np.zeros((n, len(BRANCHES)), np.int64)
+        _lib(precision).oracle_branch_signature(ctypes.byref(self.struct), n, substeps, mm_freq, float(dt), _p(q), _p(qd), _p(act), _p(musc),
+                                                h.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64)), c.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)))
+        return h, c
+
+    def exact_gradient(self, q, qd, act, musc, gq_out, gqd_out, substeps, mm_freq, dt, h=1e-30):
+        """Complex-step derivative of sum(gq_out*q' + gqd_out*qd') for ONE environment: exact to rounding (no cancellation,
+        no step-size error) for the branches the fp64 forward takes.  Returns gq, gqd, gact, gmusc (None without muscles)."""
+        d = self.desc
+        f = lambda a: np.ascontiguousarray(a, np.float64).ravel()
+        q, qd, act, gq_out, gqd_out = f(q), f(qd), f(act), f(gq_out), f(gqd_out)
+        musc = np.zeros(max(1, d.M)) if musc is None else f(musc)
+        gq, gqd, gact = np.zeros(d.Q), np.zeros(d.D), np.zeros(d.D)
+        gm = np.zeros(d.M) if d.M else None
+        _lib("c64").oracle_exact_gradient(ctypes.byref(self.struct), substeps, mm_freq, float(dt), float(h), _p(q), _p(qd), _p(act),
+                                          _p(musc), _p(gq_out), _p(gqd_out), _p(gq), _p(gqd), _p(gact), _p(gm))
+        return gq, gqd, gact, gm
 
     def fd_gradient(self, q, qd, act, musc, gq_out, gqd_out, substeps, mm_freq, dt, eps=1e-6):
         """Central differences in fp64 of sum(gq_out*q' + gqd_out*qd') for ONE environment."""
