@@ -157,6 +157,26 @@ DFX_HD Xf xf_ident() { return Xf{v3zero(), qident()}; }
 DFX_HD Xf xf_zero() { return Xf{v3zero(), qzero()}; }
 DFX_HD Xf xf_mul(Xf a, Xf b) { return Xf{qrot(a.q, b.p) + a.p, qmul(a.q, b.q)}; }
 DFX_HD V3 xf_point(Xf t, V3 x) { return t.p + qrot(t.q, x); }
+// xf_mul with every rounding spelled out as fmaf chains, for the joint-local transforms (dfx_phases.h kin_local_fwd).  Those are
+// formed in two places -- phase K1 and, with kFusedPhases, inside integrate_fwd -- that are inlined into different kernels (the
+// tape forward, the recompute adjoint).  Left to the compiler, the FMA contraction of qmul / qrot differs between those
+// contexts, and a recomputed tape row would differ from the stored one in the last bits wherever X_pj is not axis-aligned.
+DFX_HD Q4 qmul_rn(Q4 a, Q4 b) {
+    return Q4{fmaf(a.w, b.x, fmaf(b.w, a.x, fmaf(a.y, b.z, -(b.y * a.z)))),
+              fmaf(a.w, b.y, fmaf(b.w, a.y, fmaf(a.z, b.x, -(b.z * a.x)))),
+              fmaf(a.w, b.z, fmaf(b.w, a.z, fmaf(a.x, b.y, -(b.x * a.y)))),
+              fmaf(a.w, b.w, -fmaf(a.x, b.x, fmaf(a.y, b.y, a.z * b.z)))};
+}
+DFX_HD V3 qrot_rn(Q4 q, V3 x) {
+    const float k = fmaf(2.0f * q.w, q.w, -1.0f), w2 = 2.0f * q.w;
+    const float d2 = 2.0f * fmaf(q.x, x.x, fmaf(q.y, x.y, q.z * x.z));
+    const V3 c{fmaf(q.y, x.z, -(q.z * x.y)), fmaf(q.z, x.x, -(q.x * x.z)), fmaf(q.x, x.y, -(q.y * x.x))};
+    return V3{fmaf(x.x, k, fmaf(c.x, w2, q.x * d2)), fmaf(x.y, k, fmaf(c.y, w2, q.y * d2)), fmaf(x.z, k, fmaf(c.z, w2, q.z * d2))};
+}
+DFX_HD Xf xf_mul_rn(Xf a, Xf b) {
+    const V3 r = qrot_rn(a.q, b.p);
+    return Xf{V3{r.x + a.p.x, r.y + a.p.y, r.z + a.p.z}, qmul_rn(a.q, b.q)};
+}
 // c = a*b, dL/dc = r -> accumulate into aa, ab
 DFX_HD void xf_mul_adj(Xf a, Xf b, Xf r, Xf& aa, Xf& ab) {
     aa.p += r.p;

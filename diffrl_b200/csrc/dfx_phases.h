@@ -221,7 +221,7 @@ DFX_HD Xf joint_transform(const Pack& P, SP q, int i) {
 }
 
 DFX_HD void kin_local_fwd(const Pack& P, const Layout& Y, SP s, int i) {   // K1
-    st7(s + Y.Xl + i * 7, xf_mul(ld7(P.X_pj + i * 7), joint_transform(P, s + Y.q, i)));
+    st7(s + Y.Xl + i * 7, xf_mul_rn(ld7(P.X_pj + i * 7), joint_transform(P, s + Y.q, i)));   // (see xf_mul_rn)
 }
 
 // call f(p) for the links on the path root -> ... -> parent(i) [-> i], in that order (the pack lists every link's path:
@@ -353,7 +353,7 @@ DFX_HD void kin_adj_local(const Pack& P, const Layout& Y, SP s, int i) {    // A
     Xf acc = xf_zero();
     xf_mul_adj_a(ld7(s + Y.Xsc + i * 7), ld7(P.X_cm + i * 7), ld7(s + Y.aXsm + i * 7), acc);
     st7(s + Y.aXsm + i * 7, acc);                       // from here on: d/dX_sc[i] through X_sm = X_sc X_cm
-    st7(s + Y.Xl + i * 7, xf_mul(ld7(P.X_pj + i * 7), joint_transform(P, s + Y.q, i)));
+    st7(s + Y.Xl + i * 7, xf_mul_rn(ld7(P.X_pj + i * 7), joint_transform(P, s + Y.q, i)));   // (see xf_mul_rn)
     const int type = P.type[i], ds = P.qd_start[i];
     const SP qd = s + Y.qd;
     const SP S = s + Y.S;

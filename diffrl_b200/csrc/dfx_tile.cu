@@ -323,8 +323,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_kernel(const __grid_co
 // Recompute adjoint (include/dfx.h dfx_*_backward_recompute): the env-step's forward, re-run from its input state, writes the
 // tape of this tile into a caller-supplied one-env-step workspace (ka.step.tape, the tape's own layout) and the end state to
 // ka.step.q_out / qd_out (its tail); then the adjoint of dfx_tile_kernel<BACKWARD = true> reads that tape back
-// (ka.step.tape_in == ka.step.tape).  The forward is deterministic -- fixed-point scatter-adds, no float atomics -- so the
-// recomputed rows and H^-1 blocks are the stored tape's bit for bit.  Same set-up as dfx_tile_kernel (which stays as it is),
+// (ka.step.tape_in == ka.step.tape).  The forward is deterministic -- fixed-point scatter-adds, no float atomics -- and
+// the joint-local transforms, which the fused phases form inside integrate_fwd of either kernel, use explicitly rounded
+// products (dfx_math.h xf_mul_rn), so the recomputed rows and H^-1 blocks are the stored tape's bit for bit.  Same set-up as dfx_tile_kernel (which stays as it is),
 // scratch sized for the larger of the two layouts, the backward's warps and occupancy.
 template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
 __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_recompute_kernel(const __grid_constant__ KernelArgs ka) {

@@ -79,6 +79,22 @@ class ArticulationEngine:
         self.L, self.D, self.Q, self.C, self.M = desc.L, desc.D, desc.Q, desc.C, desc.M
         self.tape_bf16 = bool(self.lib.dfx_pack_query(self.pack, 10))
         self._gravity = (desc.gravity, desc.ground)
+        self._check_fits()
+
+    def _check_fits(self):
+        """The step kernels keep one environment's scratch in shared memory: refuse an articulation whose scratch does not
+        fit one CTA (227 KB), instead of failing its first launch with a bare cudaErrorInvalidConfiguration."""
+        if not hasattr(self.lib, "dfx_launch_plan"):      # (older builds loaded through DFX_LIBRARY for A/B timing)
+            return
+        plan = (ctypes.c_int * 6)()
+        for backward, what in ((0, "forward"), (1, "backward")):
+            _capi.check(self.lib.dfx_launch_plan(self.pack, backward, plan), "dfx_launch_plan")
+            if plan[1] == 0:
+                need = (self.lib.dfx_pack_query(self.pack, 5 + backward) * 4 + plan[5]) / 1024.0
+                raise _capi.DfxError(
+                    "articulation too large for the step kernels: the %s pass of one environment needs %.1f KB of shared "
+                    "memory (%d floats of scratch for L=%d links, D=%d dofs, C=%d contacts, plus the model), more than the "
+                    "227 KB of one CTA" % (what, need, self.lib.dfx_pack_query(self.pack, 5 + backward), self.L, self.D, self.C))
 
     @classmethod
     def from_model(cls, model, device, num_envs=None):
