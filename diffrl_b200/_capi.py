@@ -6,7 +6,7 @@ product entry point goes through :func:`lib`.
 import ctypes
 import os
 
-from .modelpack import DfxActionMap, DfxDerived, DfxModelDesc
+from .modelpack import DfxActionMap, DfxDerived, DfxExternalWrench, DfxModelDesc
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # DFX_LIBRARY points at another build of the SAME C ABI (same-box A/B timing of two kernel versions); never a fallback
@@ -64,6 +64,11 @@ def lib():
         L.dfx_step_backward_mapped_recompute.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
                                                          _F, _F, ctypes.POINTER(DfxActionMap), _F, _F, _F, _F, _F, _F, _F, _F, _F,
                                                          ctypes.c_void_p]
+    if hasattr(L, "dfx_step_forward_ex"):       # external wrench (include/dfx.h DfxExternalWrench); env-step entries: env_ops._bind
+        W = ctypes.POINTER(DfxExternalWrench)
+        for name in ("dfx_step_forward", "dfx_step_backward", "dfx_step_forward_mapped", "dfx_step_backward_mapped",
+                     "dfx_step_backward_recompute", "dfx_step_backward_mapped_recompute"):
+            getattr(L, name + "_ex").argtypes = getattr(L, name).argtypes + [W]
     if os.environ.get("DFX_FLAGS"):      # tuning flags of include/dfx.h (A/B runs of the test-suite)
         L.dfx_set_flags(int(os.environ["DFX_FLAGS"]))
     _lib = L

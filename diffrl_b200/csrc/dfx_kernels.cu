@@ -156,8 +156,10 @@ struct GroupCuda {
 
 // SL..SM > 0: model sizes known at compile time (the six DiffRL articulations are pre-instantiated); the scratch
 // layout and every loop bound then fold into immediates.  SL == 0: generic run-time sizes.
-template <int G, bool BACKWARD, int SL, int SD, int SQ, int SC, int SM>
-__global__ void __launch_bounds__(kMaxThreads) dfx_step_kernel(const __grid_constant__ KernelArgs ka) {
+// (instantiated twice: without and with the external wrench (WRENCH; include/dfx.h DfxExternalWrench) -- two kernels of their
+//  own, so that the ones without keep their code)
+template <int G, bool BACKWARD, int SL, int SD, int SQ, int SC, int SM, bool WRENCH>
+__device__ __forceinline__ void step_kernel_body(const KernelArgs& ka) {
     extern __shared__ __align__(16) float smem[];
     // ---- stage the model description
     float* fpack = smem;
@@ -191,8 +193,17 @@ __global__ void __launch_bounds__(kMaxThreads) dfx_step_kernel(const __grid_cons
     g.stride = ka.scratch_stride;
     g.envs_shift = 31 - __clz(kEnvsPerCta > 0 ? kEnvsPerCta : 1);
     g.cta_mode = (ka.step.flags & 8) != 0;
-    if (BACKWARD) env_step_backward(P, Y, s, g, env, ka.step);
-    else env_step_forward(P, Y, s, g, env, ka.step);
+    if (BACKWARD) env_step_backward<WRENCH>(P, Y, s, g, env, ka.step, ka.wrench);
+    else env_step_forward<WRENCH>(P, Y, s, g, env, ka.step, ka.wrench);
+}
+
+template <int G, bool BACKWARD, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(kMaxThreads) dfx_step_kernel(const __grid_constant__ KernelArgs ka) {
+    step_kernel_body<G, BACKWARD, SL, SD, SQ, SC, SM, false>(ka);
+}
+template <int G, bool BACKWARD, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(kMaxThreads) dfx_step_wrench_kernel(const __grid_constant__ KernelArgs ka) {
+    step_kernel_body<G, BACKWARD, SL, SD, SQ, SC, SM, true>(ka);
 }
 
 }  // namespace dfx
@@ -247,6 +258,7 @@ int dfx_abi_sizeof(int which) {
         case 4: return (int)sizeof(DfxActionMap);
         case 5: return (int)sizeof(DfxEnvTransition);
         case 6: return (int)sizeof(DfxEnvTransitionAdj);
+        case 7: return (int)sizeof(DfxExternalWrench);
     }
     return -1;
 }
@@ -349,9 +361,11 @@ struct LaunchPlan {
 static int cta_area(const dfx_pack* p, int envs_per_cta) {
     return 16 + ((p->header.C * envs_per_cta * 4 + 15) & ~15);
 }
-static LaunchPlan plan_launch(const dfx_pack* p, int G, bool bwd) {
+// wrench: the external-wrench kernels, whose scratch ends past the layout's (dfx_pack.h wrench_scratch_end)
+static LaunchPlan plan_launch(const dfx_pack* p, int G, bool bwd, bool wrench = false) {
     LaunchPlan lp{};
-    const int per_env = bwd ? p->host.layout_bwd.bwd_size : p->host.layout.fwd_size;
+    const int per_env = wrench ? wrench_scratch_end(bwd ? p->host.layout_bwd : p->host.layout, p->header.L, bwd)
+                               : bwd ? p->host.layout_bwd.bwd_size : p->host.layout.fwd_size;
     // multiple of 4 floats (16-byte cp.async rows) that is not a multiple of 32 (bank spreading between groups)
     lp.scratch_stride = (per_env + 3) & ~3;
     if (lp.scratch_stride % 32 == 0) lp.scratch_stride += 4;
@@ -375,14 +389,15 @@ static LaunchPlan plan_launch(const dfx_pack* p, int G, bool bwd) {
     return lp;
 }
 
-template <int G, bool BWD, int SL, int SD, int SQ, int SC, int SM>
-static cudaError_t launch_impl(const dfx_pack* p, const StepArgs& step, cudaStream_t stream) {
+template <int G, bool BWD, bool WRENCH, int SL, int SD, int SQ, int SC, int SM>
+static cudaError_t launch_impl(const dfx_pack* p, const StepArgs& step, const DfxExternalWrench& w, cudaStream_t stream) {
     KernelArgs ka;
     ka.header = p->header;
     ka.blob = p->blob;
     ka.layout = BWD ? p->host.layout_bwd : p->host.layout;
     ka.step = step;
-    const LaunchPlan lp = plan_launch(p, G, BWD);
+    ka.wrench = w;
+    const LaunchPlan lp = plan_launch(p, G, BWD, WRENCH);
     ka.scratch_stride = lp.scratch_stride;
     ka.pack_smem_floats = lp.pack_bytes / 4;
     ka.cta_area_floats = lp.cta_area_bytes / 4;
@@ -390,6 +405,7 @@ static cudaError_t launch_impl(const dfx_pack* p, const StepArgs& step, cudaStre
     if (envs_per_cta == 0) return cudaErrorInvalidConfiguration;
     const size_t smem = lp.smem;
     auto kern = dfx_step_kernel<G, BWD, SL, SD, SQ, SC, SM>;
+    if constexpr (WRENCH) kern = dfx_step_wrench_kernel<G, BWD, SL, SD, SQ, SC, SM>;
     // (the opt-in to > 48 KB of dynamic shared memory is per device: set it on every launch, it is cheap)
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -400,11 +416,11 @@ static cudaError_t launch_impl(const dfx_pack* p, const StepArgs& step, cudaStre
 }
 
 // dispatch on the model sizes: specialised instantiations for the DiffRL articulations, generic otherwise
-template <int G, bool BWD>
-static cudaError_t launch(const dfx_pack* p, const StepArgs& step, cudaStream_t stream) {
+template <int G, bool BWD, bool WRENCH>
+static cudaError_t launch(const dfx_pack* p, const StepArgs& step, const DfxExternalWrench& w, cudaStream_t stream) {
     const Pack& h = p->header;
 #define DFX_SPECIAL(l, d, q, c, m) \
-    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return launch_impl<G, BWD, l, d, q, c, m>(p, step, stream);
+    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return launch_impl<G, BWD, WRENCH, l, d, q, c, m>(p, step, w, stream);
     if (!(g_flags & 4)) {
         if constexpr (G == 16) {               // the group width pick_group() chooses for these models
             DFX_SPECIAL(9, 14, 15, 25, 0)      // Ant
@@ -418,19 +434,21 @@ static cudaError_t launch(const dfx_pack* p, const StepArgs& step, cudaStream_t 
         }
     }
 #undef DFX_SPECIAL
-    return launch_impl<G, BWD, 0, 0, 0, 0, 0>(p, step, stream);
+    return launch_impl<G, BWD, WRENCH, 0, 0, 0, 0, 0>(p, step, w, stream);
 }
 
-static cudaError_t launch_tile(const dfx_pack* p, const StepArgs& step, bool backward, cudaStream_t stream) {
+static cudaError_t launch_tile(const dfx_pack* p, const StepArgs& step, bool backward, const DfxExternalWrench* w, cudaStream_t stream) {
     KernelArgs ka;
     ka.header = p->header;
     ka.blob = p->blob;
     ka.step = step;
+    ka.wrench = w ? *w : DfxExternalWrench{nullptr, nullptr};
+    const int wr = w ? 1 : 0;
     int e = (int)cudaErrorInvalidConfiguration;
     switch (p->tile) {
-        case 8: e = dfx_tile_launch_e8(&ka, backward, stream); break;
-        case 16: e = dfx_tile_launch_e16(&ka, backward, stream); break;
-        case 32: e = dfx_tile_launch_e32(&ka, backward, stream); break;
+        case 8: e = dfx_tile_launch_e8(&ka, backward, wr, stream); break;
+        case 16: e = dfx_tile_launch_e16(&ka, backward, wr, stream); break;
+        case 32: e = dfx_tile_launch_e32(&ka, backward, wr, stream); break;
     }
     g_launches.fetch_add(1);
     return (cudaError_t)e;
@@ -442,46 +460,54 @@ static int pick_group(const dfx_pack* p) {
     return widest <= 16 ? 16 : 32;
 }
 
+template <bool WRENCH>
+static int run_group(const dfx_pack_t* p, const StepArgs& a, bool backward, const DfxExternalWrench& w, cudaStream_t st) {
+    if (backward) {
+        switch (pick_group(p)) {
+            case 8: return (int)launch<8, true, WRENCH>(p, a, w, st);
+            case 16: return (int)launch<16, true, WRENCH>(p, a, w, st);
+            default: return (int)launch<32, true, WRENCH>(p, a, w, st);
+        }
+    }
+    switch (pick_group(p)) {
+        case 8: return (int)launch<8, false, WRENCH>(p, a, w, st);
+        case 16: return (int)launch<16, false, WRENCH>(p, a, w, st);
+        default: return (int)launch<32, false, WRENCH>(p, a, w, st);
+    }
+}
+
 extern "C" {
 
 int dfx_launch_plan(const dfx_pack_t* p, int backward, int out[6]) {
     if (!p || !out) return (int)cudaErrorInvalidValue;
+    const bool bwd = (backward & 1) != 0, wrench = (backward & 2) != 0;
     if (p->tile) {      // one CTA = a tile of E environments
         KernelArgs ka;
         ka.header = p->header;
         ka.blob = p->blob;
         const size_t smem = p->tile == 8 ? dfx_tile_smem_e8(&ka, backward) : p->tile == 16 ? dfx_tile_smem_e16(&ka, backward) : dfx_tile_smem_e32(&ka, backward);
-        const Layout& Y = backward ? p->host.layout_bwd : p->host.layout;
+        const Layout& Y = bwd ? p->host.layout_bwd : p->host.layout;
         out[0] = 32; out[1] = p->tile; out[2] = (int)((227 * 1024) / (smem + 1024)); out[3] = (int)smem;
-        out[4] = ((backward ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
+        out[4] = wrench ? wrench_scratch_end(Y, p->header.L, bwd) : ((bwd ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
         out[5] = (int)smem - out[4] * p->tile * 4;
+        if (wrench && smem > 227 * 1024) out[1] = 0;      // (an articulation whose external-wrench variant no longer fits)
         return 0;
     }
     const int G = pick_group(p);
-    const LaunchPlan lp = plan_launch(p, G, backward != 0);
+    const LaunchPlan lp = plan_launch(p, G, bwd, wrench);
     out[0] = G; out[1] = lp.envs_per_cta; out[2] = lp.ctas_per_sm; out[3] = (int)lp.smem;
     out[4] = lp.scratch_stride; out[5] = lp.pack_bytes + lp.cta_area_bytes;
     return 0;
 }
 
-static int run_step(const dfx_pack_t* p, StepArgs& a, bool backward, void* stream) {
+// w: the external wrench (NULL: none -- the kernels without one)
+static int run_step(const dfx_pack_t* p, StepArgs& a, bool backward, void* stream, const DfxExternalWrench* w = nullptr) {
     a.hinv_base = tape_geom(p->header.L, p->header.Q, p->header.D, tape_envs(p, a.N), a.substeps, a.mm_freq, p->bf16 != 0).hinv_base;
     a.tape_bf16 = p->bf16;
     a.flags = g_flags;
     cudaStream_t st = (cudaStream_t)stream;
-    if (p->tile) return (int)launch_tile(p, a, backward, st);
-    if (backward) {
-        switch (pick_group(p)) {
-            case 8: return (int)launch<8, true>(p, a, st);
-            case 16: return (int)launch<16, true>(p, a, st);
-            default: return (int)launch<32, true>(p, a, st);
-        }
-    }
-    switch (pick_group(p)) {
-        case 8: return (int)launch<8, false>(p, a, st);
-        case 16: return (int)launch<16, false>(p, a, st);
-        default: return (int)launch<32, false>(p, a, st);
-    }
+    if (p->tile) return (int)launch_tile(p, a, backward, w, st);
+    return w ? run_group<true>(p, a, backward, *w, st) : run_group<false>(p, a, backward, DfxExternalWrench{nullptr, nullptr}, st);
 }
 
 static bool bind_map(const dfx_pack_t* p, const DfxActionMap* m, StepArgs& a) {
@@ -496,7 +522,13 @@ static bool bind_map(const dfx_pack_t* p, const DfxActionMap* m, StepArgs& a) {
 int dfx_step_forward(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                      const float* q, const float* qd, const float* act, const float* musc,
                      float* q_out, float* qd_out, float* tape, const DfxDerived* derived, void* stream) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0) return (int)cudaErrorInvalidValue;
+    return dfx_step_forward_ex(p, n, substeps, mm_freq, dt, q, qd, act, musc, q_out, qd_out, tape, derived, stream, nullptr);
+}
+
+int dfx_step_forward_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                        const float* q, const float* qd, const float* act, const float* musc,
+                        float* q_out, float* qd_out, float* tape, const DfxDerived* derived, void* stream, const DfxExternalWrench* w) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
     if (!q || !qd || !act || !q_out || !qd_out || (p->header.M > 0 && !musc)) return (int)cudaErrorInvalidValue;
     StepArgs a;
     memset(&a, 0, sizeof a);
@@ -504,14 +536,21 @@ int dfx_step_forward(const dfx_pack_t* p, int n, int substeps, int mm_freq, doub
     a.dt_sub = (float)(dt / (double)substeps);
     a.q = q; a.qd = qd; a.act = act; a.musc = musc; a.q_out = q_out; a.qd_out = qd_out; a.tape = tape;
     if (derived) { a.derived = *derived; a.has_derived = 1; }
-    return run_step(p, a, false, stream);
+    return run_step(p, a, false, stream, w);
 }
 
 int dfx_step_backward(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                       const float* act, const float* musc, const float* tape,
                       const float* gq_out, const float* gqd_out,
                       float* gq, float* gqd, float* gact, float* gmusc, void* stream) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !act) return (int)cudaErrorInvalidValue;
+    return dfx_step_backward_ex(p, n, substeps, mm_freq, dt, act, musc, tape, gq_out, gqd_out, gq, gqd, gact, gmusc, stream, nullptr);
+}
+
+int dfx_step_backward_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                         const float* act, const float* musc, const float* tape,
+                         const float* gq_out, const float* gqd_out,
+                         float* gq, float* gqd, float* gact, float* gmusc, void* stream, const DfxExternalWrench* w) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !act || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
     if (p->header.M > 0 && !musc) return (int)cudaErrorInvalidValue;
     StepArgs a;
     memset(&a, 0, sizeof a);
@@ -519,13 +558,20 @@ int dfx_step_backward(const dfx_pack_t* p, int n, int substeps, int mm_freq, dou
     a.dt_sub = (float)(dt / (double)substeps);
     a.act = act; a.musc = musc; a.tape_in = tape; a.gq_out = gq_out; a.gqd_out = gqd_out;
     a.gq = gq; a.gqd = gqd; a.gact = gact; a.gmusc = gmusc;
-    return run_step(p, a, true, stream);
+    return run_step(p, a, true, stream, w);
 }
 
 int dfx_step_forward_mapped(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                             const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                             float* used, float* q_out, float* qd_out, float* tape, void* stream) {
+    return dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, used, q_out, qd_out, tape, stream, nullptr);
+}
+
+int dfx_step_forward_mapped_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                               const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                               float* used, float* q_out, float* qd_out, float* tape, void* stream, const DfxExternalWrench* w) {
     if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !map || !raw || !q_out || !qd_out) return (int)cudaErrorInvalidValue;
+    if (w && !w->f_ext) return (int)cudaErrorInvalidValue;
     StepArgs a;
     memset(&a, 0, sizeof a);
     if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
@@ -534,14 +580,22 @@ int dfx_step_forward_mapped(const dfx_pack_t* p, int n, int substeps, int mm_fre
     a.dt_sub = (float)(dt / (double)substeps);
     a.q = q; a.qd = qd; a.raw = raw; a.used = used; a.q_out = q_out; a.qd_out = qd_out; a.tape = tape;
     if (a.map_muscle) a.act = act_other; else a.musc = act_other;
-    return run_step(p, a, false, stream);
+    return run_step(p, a, false, stream, w);
 }
 
 int dfx_step_backward_mapped(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                              const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
                              const float* gq_out, const float* gqd_out, const float* g_used,
                              float* gq, float* gqd, float* g_raw, void* stream) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !map || !raw) return (int)cudaErrorInvalidValue;
+    return dfx_step_backward_mapped_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, tape, gq_out, gqd_out, g_used, gq, gqd, g_raw,
+                                       stream, nullptr);
+}
+
+int dfx_step_backward_mapped_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                                const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
+                                const float* gq_out, const float* gqd_out, const float* g_used,
+                                float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* w) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !map || !raw || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
     StepArgs a;
     memset(&a, 0, sizeof a);
     if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
@@ -551,7 +605,7 @@ int dfx_step_backward_mapped(const dfx_pack_t* p, int n, int substeps, int mm_fr
     a.raw = raw; a.tape_in = tape; a.gq_out = gq_out; a.gqd_out = gqd_out; a.g_used = g_used;
     a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
     if (a.map_muscle) a.act = act_other; else a.musc = act_other;
-    return run_step(p, a, true, stream);
+    return run_step(p, a, true, stream, w);
 }
 
 // ---- env.step() as one launch (include/dfx.h): the mapped step with the transition as epilogue (tile kernels), or the two
@@ -573,12 +627,20 @@ static bool transition_ok(int kind, const DfxWalkerParams& w, const DfxPlanarPar
 int dfx_env_step_forward(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                          const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                          float* used, float* q_sim, float* qd_sim, float* tape, const DfxEnvTransition* tr, void* stream) {
+    return dfx_env_step_forward_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, used, q_sim, qd_sim, tape, tr, stream, nullptr);
+}
+
+int dfx_env_step_forward_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                            const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                            float* used, float* q_sim, float* qd_sim, float* tape, const DfxEnvTransition* tr, void* stream,
+                            const DfxExternalWrench* w) {
     if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !map || !raw || !used || !q_sim || !qd_sim || !tr) return (int)cudaErrorInvalidValue;
+    if (w && !w->f_ext) return (int)cudaErrorInvalidValue;
     if (!transition_ok(tr->kind, tr->walker, tr->planar, p, map)) return (int)cudaErrorInvalidValue;
     if (!tr->progress || !tr->start_q || !tr->start_qd || !tr->obs_before || !tr->rew || !tr->reset || !tr->q_next || !tr->qd_next ||
         !tr->actions_next || !tr->progress_next || !tr->obs_next) return (int)cudaErrorInvalidValue;
     if (!transition_fits(p, tr->kind, tr->walker, tr->planar, false)) {
-        const int e = dfx_step_forward_mapped(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, used, q_sim, qd_sim, tape, stream);
+        const int e = dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, used, q_sim, qd_sim, tape, stream, w);
         if (e != 0) return e;
         return tr->kind == 1
             ? dfx_walker_transition_forward(&tr->walker, n, q_sim, qd_sim, used, tr->progress, tr->start_q, tr->start_qd, tr->obs_before, tr->rew,
@@ -596,13 +658,19 @@ int dfx_env_step_forward(const dfx_pack_t* p, int n, int substeps, int mm_freq, 
     if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     a.env_kind = tr->kind;
     a.env = *tr;
-    return run_step(p, a, false, stream);
+    return run_step(p, a, false, stream, w);
 }
 
 int dfx_env_step_backward(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                           const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
                           const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !map || !raw || !tr) return (int)cudaErrorInvalidValue;
+    return dfx_env_step_backward_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, tape, tr, gq, gqd, g_raw, stream, nullptr);
+}
+
+int dfx_env_step_backward_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                             const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
+                             const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* w) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !map || !raw || !tr || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
     if (!transition_ok(tr->kind, tr->walker, tr->planar, p, map)) return (int)cudaErrorInvalidValue;
     if (!tr->q_sim || !tr->qd_sim || !tr->used || !tr->reset || !tr->gq_sim || !tr->gqd_sim || !tr->g_used) return (int)cudaErrorInvalidValue;
     if (!transition_fits(p, tr->kind, tr->walker, tr->planar, true)) {
@@ -612,7 +680,8 @@ int dfx_env_step_backward(const dfx_pack_t* p, int n, int substeps, int mm_freq,
             : dfx_planar_transition_backward(&tr->planar, n, tr->q_sim, tr->qd_sim, tr->used, tr->reset, tr->g_obs_before, tr->g_rew, tr->g_q_next,
                                              tr->g_qd_next, tr->g_actions_next, tr->g_obs_next, tr->gq_sim, tr->gqd_sim, tr->g_used, stream);
         if (e != 0) return e;
-        return dfx_step_backward_mapped(p, n, substeps, mm_freq, dt, map, raw, act_other, tape, tr->gq_sim, tr->gqd_sim, tr->g_used, gq, gqd, g_raw, stream);
+        return dfx_step_backward_mapped_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, tape, tr->gq_sim, tr->gqd_sim, tr->g_used, gq, gqd, g_raw,
+                                           stream, w);
     }
     StepArgs a;
     memset(&a, 0, sizeof a);
@@ -625,7 +694,7 @@ int dfx_env_step_backward(const dfx_pack_t* p, int n, int substeps, int mm_freq,
     if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     a.env_kind = tr->kind;
     a.env_adj = *tr;
-    return run_step(p, a, true, stream);
+    return run_step(p, a, true, stream, w);
 }
 
 // ---- recompute adjoint (include/dfx.h dfx_*_backward_recompute): no stored tape, the env-step's forward is re-run from its
@@ -640,7 +709,8 @@ static float* workspace_q_end(const dfx_pack_t* p, const StepArgs& a, float* ws)
 
 // one launch on the tile kernels: the forward into the workspace, the barrier sequence of dfx_tile_recompute_kernel, the adjoint.
 // `a` holds the adjoint's arguments (as the stored-tape entry would launch them); the forward's are added here.
-static int run_recompute_fused(const dfx_pack_t* p, StepArgs& a, const float* q, const float* qd, float* ws, void* stream) {
+static int run_recompute_fused(const dfx_pack_t* p, StepArgs& a, const float* q, const float* qd, float* ws, void* stream,
+                               const DfxExternalWrench* w) {
     a.q = q; a.qd = qd;
     a.q_out = workspace_q_end(p, a, ws); a.qd_out = a.q_out + (long long)a.N * p->header.Q;
     a.tape = ws; a.tape_in = ws;
@@ -652,11 +722,13 @@ static int run_recompute_fused(const dfx_pack_t* p, StepArgs& a, const float* q,
     ka.header = p->header;
     ka.blob = p->blob;
     ka.step = a;
+    ka.wrench = w ? *w : DfxExternalWrench{nullptr, nullptr};
+    const int wr = w ? 1 : 0;
     int e = (int)cudaErrorInvalidConfiguration;
     switch (p->tile) {
-        case 8: e = dfx_tile_launch_recompute_e8(&ka, stream); break;
-        case 16: e = dfx_tile_launch_recompute_e16(&ka, stream); break;
-        case 32: e = dfx_tile_launch_recompute_e32(&ka, stream); break;
+        case 8: e = dfx_tile_launch_recompute_e8(&ka, wr, stream); break;
+        case 16: e = dfx_tile_launch_recompute_e16(&ka, wr, stream); break;
+        case 32: e = dfx_tile_launch_recompute_e32(&ka, wr, stream); break;
     }
     g_launches.fetch_add(1);
     return e;
@@ -669,7 +741,15 @@ int dfx_step_backward_recompute(const dfx_pack_t* p, int n, int substeps, int mm
                                 const float* q, const float* qd, const float* act, const float* musc, float* workspace,
                                 const float* gq_out, const float* gqd_out,
                                 float* gq, float* gqd, float* gact, float* gmusc, void* stream) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !act) return (int)cudaErrorInvalidValue;
+    return dfx_step_backward_recompute_ex(p, n, substeps, mm_freq, dt, q, qd, act, musc, workspace, gq_out, gqd_out, gq, gqd, gact, gmusc,
+                                          stream, nullptr);
+}
+
+int dfx_step_backward_recompute_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                                   const float* q, const float* qd, const float* act, const float* musc, float* workspace,
+                                   const float* gq_out, const float* gqd_out,
+                                   float* gq, float* gqd, float* gact, float* gmusc, void* stream, const DfxExternalWrench* w) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !act || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
     if (p->header.M > 0 && !musc) return (int)cudaErrorInvalidValue;
     StepArgs a;
     memset(&a, 0, sizeof a);
@@ -677,20 +757,29 @@ int dfx_step_backward_recompute(const dfx_pack_t* p, int n, int substeps, int mm
     a.dt_sub = (float)(dt / (double)substeps);
     if (!recompute_fuses(p)) {
         float* q_end = workspace_q_end(p, a, workspace);
-        const int e = dfx_step_forward(p, n, substeps, mm_freq, dt, q, qd, act, musc, q_end, q_end + (long long)n * p->header.Q, workspace, nullptr, stream);
+        const int e = dfx_step_forward_ex(p, n, substeps, mm_freq, dt, q, qd, act, musc, q_end, q_end + (long long)n * p->header.Q, workspace, nullptr,
+                                          stream, w);
         if (e != 0) return e;
-        return dfx_step_backward(p, n, substeps, mm_freq, dt, act, musc, workspace, gq_out, gqd_out, gq, gqd, gact, gmusc, stream);
+        return dfx_step_backward_ex(p, n, substeps, mm_freq, dt, act, musc, workspace, gq_out, gqd_out, gq, gqd, gact, gmusc, stream, w);
     }
     a.act = act; a.musc = musc; a.gq_out = gq_out; a.gqd_out = gqd_out;
     a.gq = gq; a.gqd = gqd; a.gact = gact; a.gmusc = gmusc;
-    return run_recompute_fused(p, a, q, qd, workspace, stream);
+    return run_recompute_fused(p, a, q, qd, workspace, stream, w);
 }
 
 int dfx_step_backward_mapped_recompute(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                                        const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                                        float* workspace, const float* gq_out, const float* gqd_out, const float* g_used,
                                        float* gq, float* gqd, float* g_raw, void* stream) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !map || !raw) return (int)cudaErrorInvalidValue;
+    return dfx_step_backward_mapped_recompute_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, workspace, gq_out, gqd_out, g_used,
+                                                 gq, gqd, g_raw, stream, nullptr);
+}
+
+int dfx_step_backward_mapped_recompute_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                                          const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                                          float* workspace, const float* gq_out, const float* gqd_out, const float* g_used,
+                                          float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* w) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !map || !raw || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
     StepArgs a;
     memset(&a, 0, sizeof a);
     if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
@@ -699,21 +788,30 @@ int dfx_step_backward_mapped_recompute(const dfx_pack_t* p, int n, int substeps,
     a.dt_sub = (float)(dt / (double)substeps);
     if (!recompute_fuses(p)) {
         float* q_end = workspace_q_end(p, a, workspace);
-        const int e = dfx_step_forward_mapped(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end,
-                                              q_end + (long long)n * p->header.Q, workspace, stream);
+        const int e = dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end,
+                                                 q_end + (long long)n * p->header.Q, workspace, stream, w);
         if (e != 0) return e;
-        return dfx_step_backward_mapped(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, gq_out, gqd_out, g_used, gq, gqd, g_raw, stream);
+        return dfx_step_backward_mapped_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, gq_out, gqd_out, g_used, gq, gqd, g_raw,
+                                           stream, w);
     }
     a.raw = raw; a.gq_out = gq_out; a.gqd_out = gqd_out; a.g_used = g_used;
     a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
     if (a.map_muscle) a.act = act_other; else a.musc = act_other;
-    return run_recompute_fused(p, a, q, qd, workspace, stream);
+    return run_recompute_fused(p, a, q, qd, workspace, stream, w);
 }
 
 int dfx_env_step_backward_recompute(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                                     const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                                     float* workspace, const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream) {
+    return dfx_env_step_backward_recompute_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, workspace, tr, gq, gqd, g_raw, stream, nullptr);
+}
+
+int dfx_env_step_backward_recompute_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
+                                       const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                                       float* workspace, const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream,
+                                       const DfxExternalWrench* w) {
     if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !map || !raw || !tr) return (int)cudaErrorInvalidValue;
+    if (w && !w->f_ext) return (int)cudaErrorInvalidValue;
     if (!transition_ok(tr->kind, tr->walker, tr->planar, p, map)) return (int)cudaErrorInvalidValue;
     if (!tr->q_sim || !tr->qd_sim || !tr->used || !tr->reset || !tr->gq_sim || !tr->gqd_sim || !tr->g_used) return (int)cudaErrorInvalidValue;
     StepArgs a;
@@ -726,17 +824,17 @@ int dfx_env_step_backward_recompute(const dfx_pack_t* p, int n, int substeps, in
         // the plain mapped forward (the transition's outputs are not needed again: its adjoint reads tr->q_sim, ...), then the
         // stored-tape entry, which runs the transition adjoint as its prologue or as a launch of its own
         float* q_end = workspace_q_end(p, a, workspace);
-        const int e = dfx_step_forward_mapped(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end,
-                                              q_end + (long long)n * p->header.Q, workspace, stream);
+        const int e = dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end,
+                                                 q_end + (long long)n * p->header.Q, workspace, stream, w);
         if (e != 0) return e;
-        return dfx_env_step_backward(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, tr, gq, gqd, g_raw, stream);
+        return dfx_env_step_backward_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, tr, gq, gqd, g_raw, stream, w);
     }
     a.raw = raw; a.gq_out = tr->gq_sim; a.gqd_out = tr->gqd_sim; a.g_used = tr->g_used;
     a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
     if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     a.env_kind = tr->kind;
     a.env_adj = *tr;
-    return run_recompute_fused(p, a, q, qd, workspace, stream);
+    return run_recompute_fused(p, a, q, qd, workspace, stream, w);
 }
 
 }  // extern "C"

@@ -63,6 +63,7 @@ struct KernelArgs {
     int scratch_stride;   // floats per environment
     int pack_smem_floats; // floats reserved at the start of dynamic smem for the staged pack
     int cta_area_floats;  // then: CTA-wide task counter + task list (cta_compact)
+    DfxExternalWrench wrench;   // read by the external-wrench kernels only (last: the other fields keep their offsets)
 };
 
 
@@ -72,9 +73,11 @@ struct KernelArgs {
 // environments.  KernelArgs is a plain struct with the same layout in every build; it crosses as void*.
 #define DFX_DECLARE_TILE(E)                                                                                           \
     int dfx_tile_mode_e##E(int L, int D, int Q, int C, int M);      /* layout mode, or -1: no kernel of this width */  \
-    size_t dfx_tile_smem_e##E(const void* kernel_args, int backward); /* dynamic shared memory (bytes) */             \
-    int dfx_tile_launch_e##E(void* kernel_args, int backward, void* stream);                                         \
-    int dfx_tile_launch_recompute_e##E(void* kernel_args, void* stream);   /* forward into the workspace + adjoint, one launch */
+    /* dynamic shared memory (bytes); backward: bit 0 adjoint, bit 1 the external-wrench variant */                   \
+    size_t dfx_tile_smem_e##E(const void* kernel_args, int backward);                                                \
+    /* wrench != 0: the external-wrench kernels (kernel_args' `wrench`) */                                             \
+    int dfx_tile_launch_e##E(void* kernel_args, int backward, int wrench, void* stream);                             \
+    int dfx_tile_launch_recompute_e##E(void* kernel_args, int wrench, void* stream);   /* forward into the workspace + adjoint, one launch */
 DFX_DECLARE_TILE(8)
 DFX_DECLARE_TILE(16)
 DFX_DECLARE_TILE(32)

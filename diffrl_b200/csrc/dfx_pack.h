@@ -203,4 +203,10 @@ DFX_LAYOUT_FN Layout make_layout(int L, int D, int Q, int C, int M, int mode = k
     return y;
 }
 
+// The external-wrench variants of the step kernels (include/dfx.h DfxExternalWrench) keep two more per-environment fields
+// past the end of the layout, so every other offset stays as it is: the wrench of every link (L,6: torque, force), loaded
+// once per env-step, and in the adjoint its cotangent (L,6), accumulated over the substeps.
+DFX_LAYOUT_FN int wrench_offset(const Layout& Y, bool bwd) { return dfx_round_up(bwd ? Y.bwd_size : Y.fwd_size, 4); }
+DFX_LAYOUT_FN int wrench_scratch_end(const Layout& Y, int L, bool bwd) { return wrench_offset(Y, bwd) + dfx_round_up((bwd ? 12 : 6) * L, 4); }
+
 }  // namespace dfx

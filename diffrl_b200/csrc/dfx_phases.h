@@ -638,26 +638,39 @@ DFX_HD void inertia_apply_adj(const BodyInertia& B, SV x, SV r, M3& aR, V3& au, 
     outer_acc(aR, x.v, avb);
 }
 
-DFX_HD void body_force_link_fwd(const Pack& P, const Layout& Y, SP s, int i) {
+// kWrench: the link also feels the caller's external wrench (tau, F) at scratch offset xw (dfx_pack.h wrench_offset): a force F
+// in world axes at its centre of mass and a pure torque tau -- F enters like extra gravity, f = fb - (c x (m g + F) + tau, m g + F)
+template <bool kWrench = false>
+DFX_HD void body_force_link_fwd(const Pack& P, const Layout& Y, SP s, int i, int xw = -1) {
     const BodyInertia B = body_inertia(P, s + Y.Xsm + i * 7, i);
     const V3 c = ld3(s + Y.Xsm + i * 7);
     const SV v = ld6(s + Y.v + i * 6), a = ld6(s + Y.a + i * 6);
     const SV Ia = inertia_apply(B, a);
     const SV h = inertia_apply(B, v);
     const SV fb = Ia + sv_cross_dual(v, h);
-    const V3 mg = V3{P.gx, P.gy, P.gz} * B.m;
-    const SV fg = SV{cross(c, mg), mg};
-    st6(s + Y.f + i * 6, fb - fg);
+    if constexpr (kWrench) {
+        const SV w = ld6(s + xw + i * 6);
+        const V3 mgF = V3{P.gx, P.gy, P.gz} * B.m + w.v;
+        st6(s + Y.f + i * 6, fb - SV{cross(c, mgF) + w.w, mgF});
+    } else {
+        (void)xw;
+        const V3 mg = V3{P.gx, P.gy, P.gz} * B.m;
+        const SV fg = SV{cross(c, mg), mg};
+        st6(s + Y.f + i * 6, fb - fg);
+    }
 }
 
-template <class Grp>
-DFX_HD void body_force_fwd(const Pack& P, const Layout& Y, SP s, const Grp& g) {
-    DFX_FOR(i, P.L) body_force_link_fwd(P, Y, s, i);
+template <bool kWrench = false, class Grp>
+DFX_HD void body_force_fwd(const Pack& P, const Layout& Y, SP s, const Grp& g, int xw = -1) {
+    DFX_FOR(i, P.L) body_force_link_fwd<kWrench>(P, Y, s, i, xw);
     g.sync();
 }
 
-// adjoint: af[i] (adjoint of body_f_s[i]) plus what crba_adj left in aR[i] / au[i] -> aXsm, av, aa
-DFX_HD void body_force_link_adj(const Pack& P, const Layout& Y, SP s, int i) {
+// adjoint: af[i] (adjoint of body_f_s[i]) plus what crba_adj left in aR[i] / au[i] -> aXsm, av, aa.  kWrench: the wrench at
+// scratch offset xw enters the c cotangent as m g + F does, and its own cotangent (-af.w, -af.v + c x af.w) is added to the
+// accumulator at xw + 6 L -- one owner per link, the substeps in order: a deterministic sum
+template <bool kWrench = false>
+DFX_HD void body_force_link_adj(const Pack& P, const Layout& Y, SP s, int i, int xw = -1) {
     const SP Xsm7 = s + Y.Xsm + i * 7;
     const BodyInertia B = body_inertia(P, Xsm7, i);
     const V3 c = ld3(Xsm7);
@@ -669,8 +682,16 @@ DFX_HD void body_force_link_adj(const Pack& P, const Layout& Y, SP s, int i) {
     V3 ac = v3zero();
     SV av = sv_zero(), aa = sv_zero(), ah = sv_zero();
     // f = fb - fg ; fg = (c x mg, mg)
-    const V3 mg = V3{P.gx, P.gy, P.gz} * B.m;
-    ac += cross(mg, -af.w);
+    if constexpr (kWrench) {     // fg = (c x (mg + F) + tau, mg + F)
+        const SV w = ld6(s + xw + i * 6);
+        const V3 mgF = V3{P.gx, P.gy, P.gz} * B.m + w.v;
+        ac += cross(mgF, -af.w);
+        add6(s + xw + P.L * 6 + i * 6, SV{-af.w, cross(c, af.w) - af.v});
+    } else {
+        (void)xw;
+        const V3 mg = V3{P.gx, P.gy, P.gz} * B.m;
+        ac += cross(mg, -af.w);
+    }
     // fb = Ia + v x* h
     sv_cross_dual_adj(v, h, af, av, ah);
     inertia_apply_adj(B, v, ah, aR, au, av);
@@ -685,9 +706,9 @@ DFX_HD void body_force_link_adj(const Pack& P, const Layout& Y, SP s, int i) {
     kin_adj_local(P, Y, s, i);      // A1 of the kinematics adjoint, same link
 }
 
-template <class Grp>
-DFX_HD void body_force_adj(const Pack& P, const Layout& Y, SP s, const Grp& g) {
-    DFX_FOR(i, P.L) body_force_link_adj(P, Y, s, i);
+template <bool kWrench = false, class Grp>
+DFX_HD void body_force_adj(const Pack& P, const Layout& Y, SP s, const Grp& g, int xw = -1) {
+    DFX_FOR(i, P.L) body_force_link_adj<kWrench>(P, Y, s, i, xw);
     g.sync();
 }
 
@@ -804,10 +825,10 @@ DFX_HD void contact_fwd(const Pack& P, const Layout& Y, SP s, const Grp& g) {
 
 // rigid-body forces (dense: one item per link) and contact forces (sparse: compacted tasks) are independent: policies
 // whose barriers are CTA-wide run them as ONE phase, the link items on some warps and the contact tasks on the rest
-template <class Grp>
-DFX_HD void body_and_contact_fwd(const Pack& P, const Layout& Y, SP s, const Grp& g) {
+template <bool kWrench = false, class Grp>
+DFX_HD void body_and_contact_fwd(const Pack& P, const Layout& Y, SP s, const Grp& g, int xw = -1) {
     if (!Grp::kConcurrentItems || !P.ground) {
-        body_force_fwd(P, Y, s, g);
+        body_force_fwd<kWrench>(P, Y, s, g, xw);
         contact_fwd(P, Y, s, g);
         return;
     }
@@ -817,7 +838,7 @@ DFX_HD void body_and_contact_fwd(const Pack& P, const Layout& Y, SP s, const Grp
         const SPi lo = sp_int(se + Y.fx);
         const float c6[6] = {w.w.x, w.w.y, w.w.z, w.v.x, w.v.y, w.v.z};
         fx_scatter(lo + P.cbody[k] * 6, lo + P.L * 6 + P.cbody[k] * 6, sp_uint(se + Y.cmask), P.cbody[k], c6, kFxForward, g);
-    }, P.L, [&](SP se, int i) { body_force_link_fwd(P, Y, se, i); });
+    }, P.L, [&](SP se, int i) { body_force_link_fwd<kWrench>(P, Y, se, i, xw); });
 }
 
 template <class Grp>
@@ -1681,8 +1702,9 @@ DFX_HD void integrate_adj(const Pack& P, const Layout& Y, SP s, float dt, const 
 // adjoint of one substep.  Pre: scratch [q .. qdd] = the substep's taped block (entering q, qd and the
 // forward intermediates), act, musc, A = H^-1 of the segment; aq, aqd = cotangents of the substep output.  Post: aq, aqd = cotangents of the substep input;
 // aact, amusc, aH (Lm slot) accumulated.  `apply_crba` is set on the substep that built H.
-template <class Grp>
-DFX_HD void substep_adj(const Pack& P, const Layout& Y, SP s, float dt, bool apply_crba, HinvView hv, const RowFmt& rf, const Grp& g) {
+template <bool kWrench = false, class Grp>
+DFX_HD void substep_adj(const Pack& P, const Layout& Y, SP s, float dt, bool apply_crba, HinvView hv, const RowFmt& rf, const Grp& g,
+                        int xw = -1) {
     zero_range(s + Y.aXsc, P.L * 32 + P.D * 6, g);      // aXsc, av, aXsm, aS, aa are adjacent (af is overwritten by tau_adj)
     zero_range(s + Y.aIbar, P.L * 12, g);
     // (no barrier: integrate_adj and solve_adj do not touch the zeroed accumulators, and two barriers follow before their first use)
@@ -1702,14 +1724,14 @@ DFX_HD void substep_adj(const Pack& P, const Layout& Y, SP s, float dt, bool app
         muscle_adj(P, Y, s, scale, g);
         contact_adj(P, Y, s, g);
         adj_collect(P, Y, s, scale, g);
-        body_force_adj(P, Y, s, g);
+        body_force_adj<kWrench>(P, Y, s, g, xw);
     } else {
         // contact-only model: one item per link -- its rigid-body force adjoint, then the cotangents of its own contact points
         // in the pack's order (contacts are grouped by body, cbody_start).  Every av / aXsc entry has one writer adding in a
         // fixed order, so the sums are bit-reproducible; float atomics from compacted contact tasks would add in an order that
         // varies from run to run.  (A1 inside body_force_link_adj does not read what the contacts add.)
         DFX_FOR(i, P.L) {
-            body_force_link_adj(P, Y, s, i);
+            body_force_link_adj<kWrench>(P, Y, s, i, xw);
             if (P.ground)
                 for (int k = P.cbody_start[i]; k < P.cbody_start[i + 1]; ++k) contact_point_adj(P, Y, s, k, 1.0f, g);
         }

@@ -90,13 +90,25 @@ DFX_HD void load_actuation(const Pack& P, const Layout& Y, SP s, const Grp& g, i
     if (write_used && a.used) DFX_FOR(j, A) a.used[(long long)env * A + j] = fminf(fmaxf(re[j], -1.0f), 1.0f) * a.map_pre_scale + a.map_pre_bias;
 }
 
+// External wrench (include/dfx.h DfxExternalWrench, the _ex entries): kWrench instantiations read w.f_ext [N, L, 6] once per
+// env-step into the scratch past the layout's end (dfx_pack.h wrench_offset) and hold it over the substeps, as the actuation; the
+// adjoint writes its cotangent to w.g_f_ext (when not NULL) at the end, as gact.  The pointers travel next to StepArgs, at the
+// end of the kernel argument block, so the parameter offsets of the kernels without a wrench stay as they are.
 template <class Grp>
-DFX_HD void env_step_forward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const StepArgs& a) {
+DFX_HD void load_wrench(const Pack& P, SP s, const Grp& g, int env, const DfxExternalWrench& w, int xw) {
+    DFX_FOR(i, P.L * 6) s[xw + i] = w.f_ext[(long long)env * P.L * 6 + i];
+}
+
+template <bool kWrench = false, class Grp>
+DFX_HD void env_step_forward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const StepArgs& a,
+                             const DfxExternalWrench& w = DfxExternalWrench{nullptr, nullptr}) {
     const int Q = P.Q, D = P.D, DD = D * D;
     const RowFmt rf = row_fmt(P, Y, a.tape_bf16 != 0);
+    const int xw = kWrench ? wrench_offset(Y, false) : -1;
     DFX_FOR(i, Q) s[Y.q + i] = a.q[(long long)env * Q + i];
     DFX_FOR(i, D) s[Y.qd + i] = a.qd[(long long)env * D + i];
     load_actuation(P, Y, s, g, env, a, true);
+    if constexpr (kWrench) load_wrench(P, s, g, env, w, xw);
     for (int i = Y.qdd + D + g.lane; i < Y.q + Y.tape_row; i += Grp::G) s[i] = 0.0f;   // row padding
     if (g.lane == 0) s[Y.cmask] = 0.0f;
     DFX_FOR(i, P.L * 12) s[Y.fx + i] = 0.0f;   // fixed-point wrench accumulators (L x 6 low + high words)
@@ -113,7 +125,7 @@ DFX_HD void env_step_forward(const Pack& P, const Layout& Y, SP s, const Grp& g,
         if (a.tape) g.block_out_part(a.tape, sub, a.N, env, s + Y.q, rf, s + Y.stage, true, true);
         kin_fwd(P, Y, s, g);
         g.phase_sync();
-        body_and_contact_fwd(P, Y, s, g);
+        body_and_contact_fwd<kWrench>(P, Y, s, g, xw);
         muscle_fwd(P, Y, s, g);
         wrench_collect(P, Y, s, g);
         g.phase_sync();
@@ -146,11 +158,17 @@ DFX_HD void env_step_forward(const Pack& P, const Layout& Y, SP s, const Grp& g,
     DFX_FOR(i, D) a.qd_out[(long long)env * D + i] = s[Y.qd + i];
 }
 
-template <class Grp>
-DFX_HD void env_step_backward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const StepArgs& a) {
+template <bool kWrench = false, class Grp>
+DFX_HD void env_step_backward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const StepArgs& a,
+                              const DfxExternalWrench& w = DfxExternalWrench{nullptr, nullptr}) {
     const int Q = P.Q, D = P.D, M = P.M, DD = D * D;
     const RowFmt rf = row_fmt(P, Y, a.tape_bf16 != 0);
+    const int xw = kWrench ? wrench_offset(Y, true) : -1;
     load_actuation(P, Y, s, g, env, a, false);
+    if constexpr (kWrench) {
+        load_wrench(P, s, g, env, w, xw);
+        DFX_FOR(i, P.L * 6) s[xw + P.L * 6 + i] = 0.0f;
+    }
     DFX_FOR(i, D) s[Y.aact + i] = 0.0f;
     DFX_FOR(i, M) s[Y.amusc + i] = 0.0f;
     if (g.lane == 0) s[Y.cmask] = 0.0f;
@@ -178,7 +196,10 @@ DFX_HD void env_step_backward(const Pack& P, const Layout& Y, SP s, const Grp& g
         if constexpr (!Grp::kBulkRows) g.row_in(s + Y.q, a.tape_in, sub, a.N, env, rf.n, rf.early, rf.tail, false);
         g.copy_wait_first();
         g.sync();
-        substep_adj(P, Y, s, a.dt_sub, sub == s0, hv, rf, g);
+        substep_adj<kWrench>(P, Y, s, a.dt_sub, sub == s0, hv, rf, g, xw);
+    }
+    if constexpr (kWrench) {
+        if (w.g_f_ext) DFX_FOR(i, P.L * 6) w.g_f_ext[(long long)env * P.L * 6 + i] = s[xw + P.L * 6 + i];
     }
     if (a.gq) DFX_FOR(i, Q) a.gq[(long long)env * Q + i] = s[Y.aq + i];
     if (a.gqd) DFX_FOR(i, D) a.gqd[(long long)env * D + i] = s[Y.aqd + i];

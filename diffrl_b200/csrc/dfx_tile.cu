@@ -261,8 +261,10 @@ struct GroupTile {
     static constexpr bool kBulkRows = true;     // env_step_backward uses rows_in()
 };
 
-template <int NW, int MINB, bool BACKWARD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
-__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_kernel(const __grid_constant__ KernelArgs ka) {
+// (the kernel bodies below are instantiated twice: without and with the external wrench (WRENCH; include/dfx.h
+//  DfxExternalWrench) -- two kernels of their own, so that the ones without keep their code)
+template <int NW, bool BACKWARD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM, bool WRENCH>
+__device__ __forceinline__ void tile_kernel_body(const KernelArgs& ka) {
     constexpr int E = DFX_TILE_E;
     extern __shared__ __align__(128) float smem[];
     float* fpack = smem;
@@ -306,9 +308,9 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_kernel(const __grid_co
     // adjoint through three small global work arrays written and read by this CTA only, on either side of a CTA barrier.
     if (BACKWARD) {
         if (ka.step.env_kind) tile_transition_backward<NW * 32, E>(ka.step.env_kind, ka.step.env_adj, g.tile_base, ka.step.N);
-        env_step_backward(P, Y, s, g, env, ka.step);
+        env_step_backward<WRENCH>(P, Y, s, g, env, ka.step, ka.wrench);
     } else {
-        env_step_forward(P, Y, s, g, env, ka.step);
+        env_step_forward<WRENCH>(P, Y, s, g, env, ka.step, ka.wrench);
         if (ka.step.env_kind) {
             // the stepped state is still in the scratch tile; everything past the tape row (actuation, tau, H^-1, ...) is dead:
             // that is where the observations are formed.  `used` (global) was written by this CTA before the barrier.
@@ -320,6 +322,15 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_kernel(const __grid_co
     g.finish();
 }
 
+template <int NW, int MINB, bool BACKWARD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_kernel(const __grid_constant__ KernelArgs ka) {
+    tile_kernel_body<NW, BACKWARD, PATH, MODE, SL, SD, SQ, SC, SM, false>(ka);
+}
+template <int NW, int MINB, bool BACKWARD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_wrench_kernel(const __grid_constant__ KernelArgs ka) {
+    tile_kernel_body<NW, BACKWARD, PATH, MODE, SL, SD, SQ, SC, SM, true>(ka);
+}
+
 // Recompute adjoint (include/dfx.h dfx_*_backward_recompute): the env-step's forward, re-run from its input state, writes the
 // tape of this tile into a caller-supplied one-env-step workspace (ka.step.tape, the tape's own layout) and the end state to
 // ka.step.q_out / qd_out (its tail); then the adjoint of dfx_tile_kernel<BACKWARD = true> reads that tape back
@@ -327,8 +338,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_kernel(const __grid_co
 // the joint-local transforms, which the fused phases form inside integrate_fwd of either kernel, use explicitly rounded
 // products (dfx_math.h xf_mul_rn), so the recomputed rows and H^-1 blocks are the stored tape's bit for bit.  Same set-up as dfx_tile_kernel (which stays as it is),
 // scratch sized for the larger of the two layouts, the backward's warps and occupancy.
-template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
-__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_recompute_kernel(const __grid_constant__ KernelArgs ka) {
+template <int NW, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM, bool WRENCH>
+__device__ __forceinline__ void tile_recompute_body(const KernelArgs& ka) {
     constexpr int E = DFX_TILE_E;
     extern __shared__ __align__(128) float smem[];
     float* fpack = smem;
@@ -365,7 +376,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_recompute_kernel(const
     if (env >= ka.step.N) env = ka.step.N - 1;
     const SP s{g.tile_base + g.e};
 
-    env_step_forward(P, YF, s, g, env, ka.step);     // (no `used`, no derived dumps, no transition epilogue)
+    env_step_forward<WRENCH>(P, YF, s, g, env, ka.step, ka.wrench);     // (no `used`, no derived dumps, no transition epilogue)
     // The adjoint below reads the workspace the forward's bulk stores are still writing: TMA bulk loads of the rows (issued by
     // thread 0) and, in the layouts without a staged H^-1 (Y.A < 0: the humanoids), plain loads of H^-1 rows by every thread.
     //  1. every thread: fence its generic writes to the scratch tile against the async proxy -- the adjoint's bulk loads
@@ -382,8 +393,17 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_recompute_kernel(const
     }
     __syncthreads();
     if (ka.step.env_kind) tile_transition_backward<NW * 32, E>(ka.step.env_kind, ka.step.env_adj, g.tile_base, ka.step.N);
-    env_step_backward(P, YB, s, g, env, ka.step);
+    env_step_backward<WRENCH>(P, YB, s, g, env, ka.step, ka.wrench);
     g.finish();
+}
+
+template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_recompute_kernel(const __grid_constant__ KernelArgs ka) {
+    tile_recompute_body<NW, PATH, MODE, SL, SD, SQ, SC, SM, false>(ka);
+}
+template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_recompute_wrench_kernel(const __grid_constant__ KernelArgs ka) {
+    tile_recompute_body<NW, PATH, MODE, SL, SD, SQ, SC, SM, true>(ka);
 }
 
 // 128-byte aligned offsets so that the bulk copies of the tile stay 16-byte aligned
@@ -394,16 +414,17 @@ static int tile_pack_floats(const KernelArgs& ka) {
 // CTA area: 4 ints (task counter, cursor), 2 mbarriers (16 bytes), then one list slot per (contact point, environment)
 static int tile_area_floats(const KernelArgs& ka) { return ((32 + ka.header.C * DFX_TILE_E * 4 + 127) & ~127) / 4; }
 
-template <int NW, int MINB, bool BWD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+template <int NW, int MINB, bool BWD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM, bool WRENCH>
 static cudaError_t tile_launch_impl(KernelArgs& ka, cudaStream_t stream) {
     constexpr Layout Y = make_layout(SL, SD, SQ, SC, SM, MODE, BWD);
-    const int per_env = ((BWD ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
+    const int per_env = WRENCH ? wrench_scratch_end(Y, SL, BWD) : ((BWD ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
     ka.layout = Y;
     ka.pack_smem_floats = tile_pack_floats(ka);
     ka.cta_area_floats = tile_area_floats(ka);
     ka.scratch_stride = per_env;
     const size_t smem = (size_t)(ka.pack_smem_floats + ka.cta_area_floats + per_env * DFX_TILE_E) * sizeof(float);
     auto kern = dfx_tile_kernel<NW, MINB, BWD, PATH, MODE, SL, SD, SQ, SC, SM>;
+    if constexpr (WRENCH) kern = dfx_tile_wrench_kernel<NW, MINB, BWD, PATH, MODE, SL, SD, SQ, SC, SM>;
     // (the opt-in to > 48 KB of dynamic shared memory is per device: set it on every launch, it is cheap)
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -412,17 +433,19 @@ static cudaError_t tile_launch_impl(KernelArgs& ka, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM, bool WRENCH>
 static cudaError_t tile_recompute_launch_impl(KernelArgs& ka, cudaStream_t stream) {
     constexpr Layout YF = make_layout(SL, SD, SQ, SC, SM, MODE, false);
     constexpr Layout YB = make_layout(SL, SD, SQ, SC, SM, MODE, true);
-    const int per_env = ((YF.fwd_size > YB.bwd_size ? YF.fwd_size : YB.bwd_size) + 3) & ~3;
+    const int per_env = WRENCH ? dfx_max(wrench_scratch_end(YF, SL, false), wrench_scratch_end(YB, SL, true))
+                               : ((YF.fwd_size > YB.bwd_size ? YF.fwd_size : YB.bwd_size) + 3) & ~3;
     ka.layout = YB;
     ka.pack_smem_floats = tile_pack_floats(ka);
     ka.cta_area_floats = tile_area_floats(ka);
     ka.scratch_stride = per_env;
     const size_t smem = (size_t)(ka.pack_smem_floats + ka.cta_area_floats + per_env * DFX_TILE_E) * sizeof(float);
     auto kern = dfx_tile_recompute_kernel<NW, MINB, PATH, MODE, SL, SD, SQ, SC, SM>;
+    if constexpr (WRENCH) kern = dfx_tile_recompute_wrench_kernel<NW, MINB, PATH, MODE, SL, SD, SQ, SC, SM>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     const int ntiles = (ka.step.N + DFX_TILE_E - 1) / DFX_TILE_E;
@@ -490,21 +513,32 @@ int DFX_TILE_FN(dfx_tile_mode)(int L, int D, int Q, int C, int M) {
 size_t DFX_TILE_FN(dfx_tile_smem)(const void* kargs, int backward) {
     const KernelArgs& ka = *static_cast<const KernelArgs*>(kargs);
     const int mode = DFX_TILE_FN(dfx_tile_mode)(ka.header.L, ka.header.D, ka.header.Q, ka.header.C, ka.header.M);
-    const Layout Y = make_layout(ka.header.L, ka.header.D, ka.header.Q, ka.header.C, ka.header.M, mode < 0 ? 0 : (mode & 3), backward != 0);
-    const int per_env = ((backward ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
+    const bool bwd = (backward & 1) != 0;
+    const Layout Y = make_layout(ka.header.L, ka.header.D, ka.header.Q, ka.header.C, ka.header.M, mode < 0 ? 0 : (mode & 3), bwd);
+    const int per_env = (backward & 2) ? wrench_scratch_end(Y, ka.header.L, bwd) : ((bwd ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
     return (size_t)(tile_pack_floats(ka) + tile_area_floats(ka) + per_env * DFX_TILE_E) * sizeof(float);
 }
 
-int DFX_TILE_FN(dfx_tile_launch)(void* kargs, int backward, void* stream) {
+int DFX_TILE_FN(dfx_tile_launch)(void* kargs, int backward, int wrench, void* stream) {
     KernelArgs& ka = *static_cast<KernelArgs*>(kargs);
     const Pack& h = ka.header;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
     if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
-        return (int)(backward ? tile_launch_impl<nwb, minb, true, path, (mode) & 3, l, d, q, c, m>(ka, st)   \
-                              : tile_launch_impl<nwf, minb, false, path, (mode) & 3, l, d, q, c, m>(ka, st));
-    if (ka.step.flags & 64) { DFX_TILE_MODELS_ALT(X) }
-    DFX_TILE_MODELS(X)
+        return (int)(backward ? tile_launch_impl<nwb, minb, true, path, (mode) & 3, l, d, q, c, m, false>(ka, st)   \
+                              : tile_launch_impl<nwf, minb, false, path, (mode) & 3, l, d, q, c, m, false>(ka, st));
+    // (the flag-64 A/B variants have no external-wrench kernels: cudaErrorNotSupported below)
+    if (ka.step.flags & 64) {
+        if (wrench) return (int)cudaErrorNotSupported;
+        DFX_TILE_MODELS_ALT(X)
+    }
+    if (!wrench) { DFX_TILE_MODELS(X) }
+#undef X
+#define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
+    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
+        return (int)(backward ? tile_launch_impl<nwb, minb, true, path, (mode) & 3, l, d, q, c, m, true>(ka, st)   \
+                              : tile_launch_impl<nwf, minb, false, path, (mode) & 3, l, d, q, c, m, true>(ka, st));
+    if (wrench) { DFX_TILE_MODELS(X) }
 #undef X
     return (int)cudaErrorInvalidConfiguration;
 }
@@ -512,13 +546,14 @@ int DFX_TILE_FN(dfx_tile_launch)(void* kargs, int backward, void* stream) {
 // the recompute adjoint (dfx_tile_recompute_kernel) of every DFX_TILE_MODELS entry, with the backward kernel's warps and
 // occupancy (every entry has as many forward as backward warps; tuning builds that set them apart run the forward part with
 // the backward's).  No flag-64 (A/B) variants: the caller runs the forward and the backward launches instead.
-int DFX_TILE_FN(dfx_tile_launch_recompute)(void* kargs, void* stream) {
+int DFX_TILE_FN(dfx_tile_launch_recompute)(void* kargs, int wrench, void* stream) {
     KernelArgs& ka = *static_cast<KernelArgs*>(kargs);
     const Pack& h = ka.header;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
     if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
-        return (int)tile_recompute_launch_impl<nwb, minb, path, (mode) & 3, l, d, q, c, m>(ka, st);
+        return (int)(wrench ? tile_recompute_launch_impl<nwb, minb, path, (mode) & 3, l, d, q, c, m, true>(ka, st)   \
+                            : tile_recompute_launch_impl<nwb, minb, path, (mode) & 3, l, d, q, c, m, false>(ka, st));
     DFX_TILE_MODELS(X)
 #undef X
     return (int)cudaErrorInvalidConfiguration;

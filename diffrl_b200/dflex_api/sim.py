@@ -6,6 +6,9 @@ substeps of ``dt/substeps`` with the actuation held constant, the joint-space in
 every ``mass_matrix_freq`` substeps, gradients flowing to ``state_in.joint_q / joint_qd / joint_act``
 and ``model.muscle_activation``.  Underneath, one fused sm_90a kernel per env-step (and one for its
 adjoint) replaces the reference's tape of 10-11 generated kernels per substep.
+
+``state_in.body_f_ext`` (optional, [N*L, 6] or [N, L, 6]): external link wrenches (torque, force at the centre of mass, world
+axes; include/dfx.h DfxExternalWrench) held over the env-step's substeps, differentiable.  A returned State carries none.
 """
 import torch
 
@@ -61,7 +64,8 @@ def _derived_getattr(self, name):
         self.__dict__["_derive_ctx"] = (engine, q, qd, act, drive if is_muscle else None, substeps, mm_freq, dt)
     if name in _DERIVED and "_derive_ctx" in self.__dict__:
         engine, q, qd, act, musc, substeps, mm_freq, dt = self.__dict__["_derive_ctx"]
-        _, _, _, dumps = engine.forward(q, qd, act, musc, substeps, mm_freq, dt, want_tape=False, derived=list(_DERIVED))
+        _, _, _, dumps = engine.forward(q, qd, act, musc, substeps, mm_freq, dt, want_tape=False, derived=list(_DERIVED),
+                                        f_ext=self.__dict__.get("_derive_f_ext"))
         for key, value in dumps.items():
             self.__dict__[key] = value
         return self.__dict__[name]
@@ -71,20 +75,32 @@ def _derived_getattr(self, name):
 State.__getattr__ = _derived_getattr
 
 
+def _wrench_in(state):
+    """``state.body_f_ext`` when set (no derived-field lookup)."""
+    return state.__dict__.get("body_f_ext")
+
+
+def _wrench_args(f_ext):
+    return () if f_ext is None else (f_ext,)
+
+
 def fused_mapped_forward(model, state_in, dt, substeps, mass_matrix_freq, raw_actions, amap):
     """``SemiImplicitIntegrator.forward`` with the env's action map folded into the launch (the env layer's fast path,
     ``envs/base.py:_fused_step``): returns (State, used) where ``used`` are the clipped / affinely mapped actions.
-    ``amap`` = (offset, pre_scale, pre_bias, drive_scale, strength, is_muscle)."""
+    ``amap`` = (offset, pre_scale, pre_bias, drive_scale, strength, is_muscle).  Reads ``state_in.body_f_ext``."""
     from ..engine import MappedSimStepFunction
     engine = _engine_for(model)
+    f_ext = _wrench_in(state_in)
     q_new, qd_new, used = MappedSimStepFunction.apply(engine, int(substeps), int(mass_matrix_freq), float(dt), amap,
-                                                      state_in.joint_q, state_in.joint_qd, raw_actions)
+                                                      state_in.joint_q, state_in.joint_qd, raw_actions, *_wrench_args(f_ext))
     out = State()
     out.particle_count, out.link_count = model.particle_count, model.link_count
     out.joint_q, out.joint_qd = q_new, qd_new
     out.__dict__["_act_proto"] = model.joint_qd
     out.__dict__["_derive_ctx_mapped"] = (engine, state_in.joint_q.detach(), state_in.joint_qd.detach(), raw_actions.detach(), amap,
                                           int(substeps), int(mass_matrix_freq), float(dt))
+    if f_ext is not None:
+        out.__dict__["_derive_f_ext"] = f_ext.detach()
     return out, used
 
 
@@ -92,18 +108,21 @@ def fused_env_step(model, state_in, dt, substeps, mass_matrix_freq, raw_actions,
     """env.step() as one launch (``env_ops.EnvStepFunction`` over ``dfx_env_step_forward / _backward``): the simulation step with
     the action map folded in and the env transition as its epilogue.  Returns (State of the NEXT step's start, (obs_before_reset,
     rew, reset, actions_next, progress_next, obs_next)).  ``nan_guard``: non-finite cotangents of (q, qd, actions) become 0
-    (the reference's humanoid.py:196-206 hooks)."""
+    (the reference's humanoid.py:196-206 hooks; the wrench's cotangent too).  Reads ``state_in.body_f_ext``."""
     from ..env_ops import EnvStepFunction
     engine = _engine_for(model)
+    f_ext = _wrench_in(state_in)
     (obs_before, rew, reset, q_next, qd_next, actions_next, progress_next, obs_next) = EnvStepFunction.apply(
         engine, int(substeps), int(mass_matrix_freq), float(dt), amap, tparams, bool(nan_guard), progress, start_q, start_qd,
-        state_in.joint_q, state_in.joint_qd, raw_actions)
+        state_in.joint_q, state_in.joint_qd, raw_actions, *_wrench_args(f_ext))
     out = State()
     out.particle_count, out.link_count = model.particle_count, model.link_count
     out.joint_q, out.joint_qd = q_next.view(-1), qd_next.view(-1)
     out.__dict__["_act_proto"] = model.joint_qd
     out.__dict__["_derive_ctx_mapped"] = (engine, state_in.joint_q.detach(), state_in.joint_qd.detach(), raw_actions.detach(), amap,
                                           int(substeps), int(mass_matrix_freq), float(dt))
+    if f_ext is not None:
+        out.__dict__["_derive_f_ext"] = f_ext.detach()
     return out, (obs_before, rew, reset, actions_next, progress_next, obs_next)
 
 
@@ -116,19 +135,20 @@ class SemiImplicitIntegrator:
     def forward(self, model, state_in, dt, substeps, mass_matrix_freq):
         engine = _engine_for(model)
         musc = model.muscle_activation if engine.M else None
+        f_ext = _wrench_in(state_in)
         if config.no_grad:
             with torch.no_grad():
                 q = state_in.joint_q if state_in.joint_q.is_contiguous() else state_in.joint_q.contiguous()
                 qd = state_in.joint_qd if state_in.joint_qd.is_contiguous() else state_in.joint_qd.contiguous()
                 engine.forward(q, qd, state_in.joint_act, musc, substeps, mass_matrix_freq, dt,
-                               want_tape=False, out=(q.view(-1), qd.view(-1)))
+                               want_tape=False, out=(q.view(-1), qd.view(-1)), f_ext=f_ext)
                 if q is not state_in.joint_q:
                     state_in.joint_q.copy_(q)
                     state_in.joint_qd.copy_(qd)
             return state_in
         from ..engine import SimStepFunction
         q_new, qd_new = SimStepFunction.apply(engine, int(substeps), int(mass_matrix_freq), float(dt),
-                                              state_in.joint_q, state_in.joint_qd, state_in.joint_act, musc)
+                                              state_in.joint_q, state_in.joint_qd, state_in.joint_act, musc, *_wrench_args(f_ext))
         out = State()
         out.particle_count, out.link_count = model.particle_count, model.link_count
         out.joint_q, out.joint_qd = q_new, qd_new
@@ -136,6 +156,8 @@ class SemiImplicitIntegrator:
         out.__dict__["_derive_ctx"] = (engine, state_in.joint_q.detach(), state_in.joint_qd.detach(),
                                        state_in.joint_act.detach(), None if musc is None else musc.detach(),
                                        int(substeps), int(mass_matrix_freq), float(dt))
+        if f_ext is not None:
+            out.__dict__["_derive_f_ext"] = f_ext.detach()
         if config.verify_fp:
             assert torch.isfinite(q_new).all() and torch.isfinite(qd_new).all(), "non-finite state after integration"
         return out

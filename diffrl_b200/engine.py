@@ -16,7 +16,7 @@ import ctypes
 import torch
 
 from . import _capi
-from .modelpack import DfxDerived, articulation_from_model
+from .modelpack import DfxDerived, DfxExternalWrench, articulation_from_model
 
 _DERIVED_SHAPES = {
     "body_X_sc": ("L", 7), "body_X_sm": ("L", 7), "joint_S_s": ("D", 6), "body_v_s": ("L", 6),
@@ -41,6 +41,32 @@ def _f32c(t, device):
     if t.dtype != torch.float32 or t.device != device or not t.is_contiguous():
         t = t.to(device=device, dtype=torch.float32).contiguous()
     return t
+
+
+def check_wrench(engine, f_ext):
+    """``f_ext``: per-environment external link wrenches, [N, L, 6] or [N*L, 6] fp32 on the engine's device -- row (e, i) is
+    (torque, force), both in world axes, the force applied at link i's centre of mass (include/dfx.h DfxExternalWrench).
+    Returns it detached and contiguous (None stays None); anything else is a ValueError."""
+    if f_ext is None:
+        return None
+    if not isinstance(f_ext, torch.Tensor):
+        raise ValueError("f_ext must be a torch.Tensor, got %s" % type(f_ext).__name__)
+    if f_ext.dtype != torch.float32:
+        raise ValueError("f_ext must be float32, got %s" % f_ext.dtype)
+    if f_ext.device != engine.device:
+        raise ValueError("f_ext is on %s, the engine on %s" % (f_ext.device, engine.device))
+    if tuple(f_ext.shape) not in ((engine.N, engine.L, 6), (engine.N * engine.L, 6)):
+        raise ValueError("f_ext has shape %s, expected [%d, %d, 6] or [%d, 6]" % (tuple(f_ext.shape), engine.N, engine.L,
+                                                                                  engine.N * engine.L))
+    engine.check_wrench_fits()
+    return f_ext.detach().contiguous()
+
+
+def wrench_struct(f_ext, g_f_ext=None):
+    """The DfxExternalWrench of an _ex entry (by reference), or None: no wrench."""
+    if f_ext is None:
+        return None
+    return ctypes.byref(DfxExternalWrench(f_ext.data_ptr(), None if g_f_ext is None else g_f_ext.data_ptr()))
 
 
 _GRAVEYARD = []
@@ -79,22 +105,37 @@ class ArticulationEngine:
         self.L, self.D, self.Q, self.C, self.M = desc.L, desc.D, desc.Q, desc.C, desc.M
         self.tape_bf16 = bool(self.lib.dfx_pack_query(self.pack, 10))
         self._gravity = (desc.gravity, desc.ground)
+        self._wrench_fits = False
         self._check_fits()
 
-    def _check_fits(self):
+    def _check_fits(self, wrench=False):
         """The step kernels keep one environment's scratch in shared memory: refuse an articulation whose scratch does not
-        fit one CTA (227 KB), instead of failing its first launch with a bare cudaErrorInvalidConfiguration."""
+        fit one CTA (227 KB), instead of failing its first launch with a bare cudaErrorInvalidConfiguration.  ``wrench``: the
+        external-wrench kernels, whose scratch holds the wrench and its cotangent as well."""
         if not hasattr(self.lib, "dfx_launch_plan"):      # (older builds loaded through DFX_LIBRARY for A/B timing)
             return
         plan = (ctypes.c_int * 6)()
         for backward, what in ((0, "forward"), (1, "backward")):
-            _capi.check(self.lib.dfx_launch_plan(self.pack, backward, plan), "dfx_launch_plan")
+            _capi.check(self.lib.dfx_launch_plan(self.pack, backward | (2 if wrench else 0), plan), "dfx_launch_plan")
             if plan[1] == 0:
-                need = (self.lib.dfx_pack_query(self.pack, 5 + backward) * 4 + plan[5]) / 1024.0
+                floats = self.lib.dfx_pack_query(self.pack, 5 + backward)
+                extra = ""
+                if wrench:
+                    floats = int(plan[4])
+                    extra = " with the external wrench and its cotangent staged"
+                need = (floats * 4 + plan[5]) / 1024.0
                 raise _capi.DfxError(
-                    "articulation too large for the step kernels: the %s pass of one environment needs %.1f KB of shared "
+                    "articulation too large for the step kernels%s: the %s pass of one environment needs %.1f KB of shared "
                     "memory (%d floats of scratch for L=%d links, D=%d dofs, C=%d contacts, plus the model), more than the "
-                    "227 KB of one CTA" % (what, need, self.lib.dfx_pack_query(self.pack, 5 + backward), self.L, self.D, self.C))
+                    "227 KB of one CTA" % (extra, what, need, floats, self.L, self.D, self.C))
+
+    def check_wrench_fits(self):
+        """Raise DfxError when the external-wrench kernels of this articulation do not fit one CTA (checked once)."""
+        if not self._wrench_fits:
+            if not hasattr(self.lib, "dfx_step_forward_ex"):
+                raise _capi.DfxError("%s has no external-wrench entries (dfx_*_ex)" % _capi.LIB_PATH)
+            self._check_fits(wrench=True)
+            self._wrench_fits = True
 
     @classmethod
     def from_model(cls, model, device, num_envs=None):
@@ -163,10 +204,12 @@ class ArticulationEngine:
     def _stream(self):
         return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
-    def forward(self, q, qd, act, musc, substeps, mm_freq, dt, want_tape=True, derived=None, out=None):
+    def forward(self, q, qd, act, musc, substeps, mm_freq, dt, want_tape=True, derived=None, out=None, f_ext=None):
         """Returns (q_out, qd_out, tape or None).  ``derived``: optional dict name -> bool of dumps to
-        fill (returned as a dict of tensors under key 'derived' attribute of the result tuple)."""
+        fill (returned as a dict of tensors under key 'derived' attribute of the result tuple).  ``f_ext``: external link
+        wrenches [N, L, 6] (``check_wrench``), held over the substeps; the backward must be given the same."""
         dev = self.device
+        f_ext = check_wrench(self, f_ext)
         q, qd, act = _f32c(q, dev), _f32c(qd, dev), _f32c(act, dev)
         if q.numel() != self.N * self.Q or qd.numel() != self.N * self.D or act.numel() != self.N * self.D:
             raise ValueError("state tensors do not match num_envs=%d, Q=%d, D=%d" % (self.N, self.Q, self.D))
@@ -192,15 +235,26 @@ class ArticulationEngine:
                 shape = (self.N * dims[a], b) if b else (self.N * dims[a],)
                 dumps[name] = torch.zeros(shape, dtype=torch.float32, device=dev)
                 setattr(dv, name, dumps[name].data_ptr())
+        args = (self.pack, self.N, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd), _ptr(act), _ptr(musc), _ptr(q_out),
+                _ptr(qd_out), _ptr(tape), None if dv is None else ctypes.byref(dv), self._stream())
         with torch.cuda.device(dev):
-            code = self.lib.dfx_step_forward(self.pack, self.N, int(substeps), int(mm_freq), float(dt),
-                                             _ptr(q), _ptr(qd), _ptr(act), _ptr(musc), _ptr(q_out), _ptr(qd_out),
-                                             _ptr(tape), None if dv is None else ctypes.byref(dv), self._stream())
+            if f_ext is None:
+                code = self.lib.dfx_step_forward(*args)
+            else:
+                code = self.lib.dfx_step_forward_ex(*args, wrench_struct(f_ext))
         _capi.check(code, "dfx_step_forward")
         return q_out, qd_out, tape, dumps
 
-    def backward(self, act, musc, tape, gq_out, gqd_out, substeps, mm_freq, dt, need=(True, True, True, True)):
+    def _wrench_grad(self, f_ext, need):
+        return torch.empty(f_ext.shape, dtype=torch.float32, device=self.device) if (f_ext is not None and need) else None
+
+    def backward(self, act, musc, tape, gq_out, gqd_out, substeps, mm_freq, dt, need=(True, True, True, True), f_ext=None,
+                 need_f_ext=True):
+        """Cotangents (gq, gqd, gact, gmusc) of the inputs; with ``f_ext`` (the forward's) a fifth, g_f_ext (None unless
+        ``need_f_ext``), shaped as ``f_ext``."""
         dev = self.device
+        f_ext = check_wrench(self, f_ext)
+        g_f_ext = self._wrench_grad(f_ext, need_f_ext)
         act = _f32c(act, dev)
         musc = _f32c(musc, dev) if self.M else None
         gq_out = None if gq_out is None else _f32c(gq_out, dev)
@@ -209,19 +263,26 @@ class ArticulationEngine:
         gqd = torch.empty(self.N * self.D, dtype=torch.float32, device=dev) if need[1] else None
         gact = torch.empty(self.N * self.D, dtype=torch.float32, device=dev) if need[2] else None
         gmusc = torch.empty(self.N * self.M, dtype=torch.float32, device=dev) if (need[3] and self.M) else None
+        args = (self.pack, self.N, int(substeps), int(mm_freq), float(dt), _ptr(act), _ptr(musc), _ptr(tape), _ptr(gq_out),
+                _ptr(gqd_out), _ptr(gq), _ptr(gqd), _ptr(gact), _ptr(gmusc), self._stream())
         with torch.cuda.device(dev):
-            code = self.lib.dfx_step_backward(self.pack, self.N, int(substeps), int(mm_freq), float(dt),
-                                              _ptr(act), _ptr(musc), _ptr(tape), _ptr(gq_out), _ptr(gqd_out),
-                                              _ptr(gq), _ptr(gqd), _ptr(gact), _ptr(gmusc), self._stream())
+            if f_ext is None:
+                code = self.lib.dfx_step_backward(*args)
+            else:
+                code = self.lib.dfx_step_backward_ex(*args, wrench_struct(f_ext, g_f_ext))
         _capi.check(code, "dfx_step_backward")
-        return gq, gqd, gact, gmusc
+        if f_ext is None:
+            return gq, gqd, gact, gmusc
+        return gq, gqd, gact, gmusc, g_f_ext
 
     def backward_recompute(self, q, qd, act, musc, gq_out, gqd_out, substeps, mm_freq, dt, need=(True, True, True, True),
-                           workspace=None):
-        """``backward`` without a tape: the env-step's forward from (q, qd, act, musc) is re-run into a workspace inside the
-        adjoint launch (``dfx_step_backward_recompute``).  ``workspace`` (``recompute_workspace()``): used and left readable
+                           workspace=None, f_ext=None, need_f_ext=True):
+        """``backward`` without a tape: the env-step's forward from (q, qd, act, musc[, f_ext]) is re-run into a workspace inside
+        the adjoint launch (``dfx_step_backward_recompute``).  ``workspace`` (``recompute_workspace()``): used and left readable
         (``tape_rows``, ``tape_hinv``, ``workspace_end_state``); None: one from the caching allocator."""
         dev = self.device
+        f_ext = check_wrench(self, f_ext)
+        g_f_ext = self._wrench_grad(f_ext, need_f_ext)
         q, qd, act = _f32c(q, dev), _f32c(qd, dev), _f32c(act, dev)
         musc = _f32c(musc, dev) if self.M else None
         gq_out = None if gq_out is None else _f32c(gq_out, dev)
@@ -232,47 +293,56 @@ class ArticulationEngine:
         gqd = torch.empty(self.N * self.D, dtype=torch.float32, device=dev) if need[1] else None
         gact = torch.empty(self.N * self.D, dtype=torch.float32, device=dev) if need[2] else None
         gmusc = torch.empty(self.N * self.M, dtype=torch.float32, device=dev) if (need[3] and self.M) else None
+        args = (self.pack, self.N, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd), _ptr(act), _ptr(musc), _ptr(workspace),
+                _ptr(gq_out), _ptr(gqd_out), _ptr(gq), _ptr(gqd), _ptr(gact), _ptr(gmusc), self._stream())
         with torch.cuda.device(dev):
-            code = self.lib.dfx_step_backward_recompute(self.pack, self.N, int(substeps), int(mm_freq), float(dt),
-                                                        _ptr(q), _ptr(qd), _ptr(act), _ptr(musc), _ptr(workspace),
-                                                        _ptr(gq_out), _ptr(gqd_out), _ptr(gq), _ptr(gqd), _ptr(gact), _ptr(gmusc),
-                                                        self._stream())
+            if f_ext is None:
+                code = self.lib.dfx_step_backward_recompute(*args)
+            else:
+                code = self.lib.dfx_step_backward_recompute_ex(*args, wrench_struct(f_ext, g_f_ext))
         _capi.check(code, "dfx_step_backward_recompute")
-        return gq, gqd, gact, gmusc
+        if f_ext is None:
+            return gq, gqd, gact, gmusc
+        return gq, gqd, gact, gmusc, g_f_ext
 
 
 class MappedSimStepFunction(torch.autograd.Function):
     """(q, qd, raw policy output) -> (q', qd', used): the env-step with the action map folded into the simulation launch
     (``dfx_step_forward_mapped`` / ``dfx_step_backward_mapped``): ``used = clip(raw, -1, 1) * pre_scale + pre_bias`` (the env's
     ``actions``), ``joint_act`` / the muscle activations are formed inside the kernel.  ``amap`` = (offset, pre_scale, pre_bias,
-    drive_scale, strength [A], is_muscle)."""
+    drive_scale, strength [A], is_muscle).  ``f_ext``: optional external link wrenches [N, L, 6] (``check_wrench``); its
+    gradient is returned when it requires one."""
 
     @staticmethod
-    def forward(ctx, engine, substeps, mm_freq, dt, amap, q, qd, raw):
+    def forward(ctx, engine, substeps, mm_freq, dt, amap, q, qd, raw, f_ext=None):
         from .modelpack import DfxActionMap
         offset, pre_scale, pre_bias, drive_scale, strength, is_muscle = amap
         dev = engine.device
         q, qd = _f32c(q.detach(), dev), _f32c(qd.detach(), dev)
         raw = _f32c(raw.detach(), dev)
+        f_ext = check_wrench(engine, f_ext)
         n, A = engine.N, raw.shape[-1]
         m = DfxActionMap(int(A), int(offset), int(bool(is_muscle)), float(pre_scale), float(pre_bias), float(drive_scale), strength.data_ptr())
-        need = any(ctx.needs_input_grad[5:8])
+        need = any(ctx.needs_input_grad[5:9])
         ctx.recompute = recompute_adjoint()
         q_out, qd_out, used = torch.empty_like(q), torch.empty_like(qd), torch.empty_like(raw)
         tape = torch.empty(engine.tape_floats(substeps, mm_freq), dtype=torch.float32, device=dev) if (need and not ctx.recompute) else None
+        args = (engine.pack, n, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd), ctypes.byref(m), _ptr(raw), None, _ptr(used),
+                _ptr(q_out), _ptr(qd_out), _ptr(tape), engine._stream())
         with torch.cuda.device(dev):
-            code = engine.lib.dfx_step_forward_mapped(engine.pack, n, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd),
-                                                      ctypes.byref(m), _ptr(raw), None, _ptr(used), _ptr(q_out), _ptr(qd_out),
-                                                      _ptr(tape), engine._stream())
+            if f_ext is None:
+                code = engine.lib.dfx_step_forward_mapped(*args)
+            else:
+                code = engine.lib.dfx_step_forward_mapped_ex(*args, wrench_struct(f_ext))
         _capi.check(code, "dfx_step_forward_mapped")
         ctx.engine, ctx.cfg, ctx.amap = engine, (substeps, mm_freq, dt), m
         ctx.strength = strength                      # keeps the device array the struct points at alive
         ctx.set_materialize_grads(False)
         ctx.shapes = (q.shape, qd.shape)
         if ctx.recompute:
-            ctx.save_for_backward(raw, q, qd)        # the env-step's input state, in place of its tape
+            ctx.save_for_backward(raw, f_ext, q, qd)        # the env-step's input state, in place of its tape
         else:
-            ctx.save_for_backward(raw, tape)
+            ctx.save_for_backward(raw, f_ext, tape)
         return q_out, qd_out, used
 
     @staticmethod
@@ -286,57 +356,75 @@ class MappedSimStepFunction(torch.autograd.Function):
         gqd = torch.empty(engine.N * engine.D, dtype=torch.float32, device=dev)
         cot = (_ptr(gq_out), _ptr(gqd_out), _ptr(g_used), _ptr(gq), _ptr(gqd))
         if ctx.recompute:
-            raw, q, qd = ctx.saved_tensors
+            raw, f_ext, q, qd = ctx.saved_tensors
             g_raw = torch.empty_like(raw)
+            g_f_ext = engine._wrench_grad(f_ext, ctx.needs_input_grad[8] if f_ext is not None else False)
             workspace = engine.recompute_workspace(substeps, mm_freq)
+            args = (engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd), ctypes.byref(ctx.amap), _ptr(raw), None,
+                    _ptr(workspace), *cot, _ptr(g_raw), engine._stream())
             with torch.cuda.device(dev):
-                code = engine.lib.dfx_step_backward_mapped_recompute(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt),
-                                                                     _ptr(q), _ptr(qd), ctypes.byref(ctx.amap), _ptr(raw), None,
-                                                                     _ptr(workspace), *cot, _ptr(g_raw), engine._stream())
+                if f_ext is None:
+                    code = engine.lib.dfx_step_backward_mapped_recompute(*args)
+                else:
+                    code = engine.lib.dfx_step_backward_mapped_recompute_ex(*args, wrench_struct(f_ext, g_f_ext))
             _capi.check(code, "dfx_step_backward_mapped_recompute")
         else:
-            raw, tape = ctx.saved_tensors
+            raw, f_ext, tape = ctx.saved_tensors
             g_raw = torch.empty_like(raw)
+            g_f_ext = engine._wrench_grad(f_ext, ctx.needs_input_grad[8] if f_ext is not None else False)
+            args = (engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), ctypes.byref(ctx.amap), _ptr(raw), None, _ptr(tape), *cot,
+                    _ptr(g_raw), engine._stream())
             with torch.cuda.device(dev):
-                code = engine.lib.dfx_step_backward_mapped(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), ctypes.byref(ctx.amap),
-                                                           _ptr(raw), None, _ptr(tape), *cot, _ptr(g_raw), engine._stream())
+                if f_ext is None:
+                    code = engine.lib.dfx_step_backward_mapped(*args)
+                else:
+                    code = engine.lib.dfx_step_backward_mapped_ex(*args, wrench_struct(f_ext, g_f_ext))
             _capi.check(code, "dfx_step_backward_mapped")
-        return None, None, None, None, None, gq.view(ctx.shapes[0]), gqd.view(ctx.shapes[1]), g_raw
+        return None, None, None, None, None, gq.view(ctx.shapes[0]), gqd.view(ctx.shapes[1]), g_raw, g_f_ext
 
 
 class SimStepFunction(torch.autograd.Function):
-    """(q, qd, act, musc) -> (q', qd') for one env-step; the drop-in for the reference SimulateFunc."""
+    """(q, qd, act, musc[, f_ext]) -> (q', qd') for one env-step; the drop-in for the reference SimulateFunc.  ``f_ext``: optional
+    external link wrenches [N, L, 6] (``check_wrench``); its gradient is returned when it requires one."""
 
     @staticmethod
-    def forward(ctx, engine, substeps, mm_freq, dt, q, qd, act, musc):
+    def forward(ctx, engine, substeps, mm_freq, dt, q, qd, act, musc, f_ext=None):
         needs = ctx.needs_input_grad[4:8]
+        ctx.need_f_ext = len(ctx.needs_input_grad) > 8 and ctx.needs_input_grad[8]
         ctx.recompute = recompute_adjoint()
+        f_ext = check_wrench(engine, f_ext)
         q_out, qd_out, tape, _ = engine.forward(q.detach(), qd.detach(), act.detach(),
                                                 None if musc is None else musc.detach(),
-                                                substeps, mm_freq, dt, want_tape=any(needs) and not ctx.recompute)
+                                                substeps, mm_freq, dt, want_tape=(any(needs) or ctx.need_f_ext) and not ctx.recompute,
+                                                f_ext=f_ext)
         ctx.engine, ctx.cfg, ctx.needs = engine, (substeps, mm_freq, dt), needs
         ctx.set_materialize_grads(False)      # a missing cotangent is NULL for dfx_step_backward, not a zero fill
         ctx.shapes = (q.shape, qd.shape, act.shape, None if musc is None else musc.shape)
         musc = musc.detach() if (musc is not None and engine.M) else None
         if ctx.recompute:
-            ctx.save_for_backward(act.detach(), musc, q.detach(), qd.detach())   # the env-step's input state, in place of its tape
+            ctx.save_for_backward(act.detach(), musc, f_ext, q.detach(), qd.detach())   # the env-step's input state, in place of its tape
         else:
-            ctx.save_for_backward(act.detach(), musc, tape)
+            ctx.save_for_backward(act.detach(), musc, f_ext, tape)
         return q_out.view(q.shape), qd_out.view(qd.shape)
 
     @staticmethod
     def backward(ctx, gq_out, gqd_out):
         substeps, mm_freq, dt = ctx.cfg
+        wrench = dict(f_ext=None)
         if ctx.recompute:
-            act, musc, q, qd = ctx.saved_tensors
-            gq, gqd, gact, gmusc = ctx.engine.backward_recompute(q, qd, act, musc, gq_out, gqd_out, substeps, mm_freq, dt,
-                                                                 need=tuple(ctx.needs))
+            act, musc, f_ext, q, qd = ctx.saved_tensors
+            if f_ext is not None:
+                wrench = dict(f_ext=f_ext, need_f_ext=ctx.need_f_ext)
+            g = ctx.engine.backward_recompute(q, qd, act, musc, gq_out, gqd_out, substeps, mm_freq, dt, need=tuple(ctx.needs), **wrench)
         else:
-            act, musc, tape = ctx.saved_tensors
-            gq, gqd, gact, gmusc = ctx.engine.backward(act, musc, tape, gq_out, gqd_out, substeps, mm_freq, dt,
-                                                       need=tuple(ctx.needs))
+            act, musc, f_ext, tape = ctx.saved_tensors
+            if f_ext is not None:
+                wrench = dict(f_ext=f_ext, need_f_ext=ctx.need_f_ext)
+            g = ctx.engine.backward(act, musc, tape, gq_out, gqd_out, substeps, mm_freq, dt, need=tuple(ctx.needs), **wrench)
+        gq, gqd, gact, gmusc = g[:4]
+        g_f_ext = g[4] if len(g) > 4 else None
         sq, sqd, sact, smusc = ctx.shapes
         return (None, None, None, None,
                 None if gq is None else gq.view(sq), None if gqd is None else gqd.view(sqd),
                 None if gact is None else gact.view(sact),
-                None if (gmusc is None or smusc is None) else gmusc.view(smusc))
+                None if (gmusc is None or smusc is None) else gmusc.view(smusc), g_f_ext)

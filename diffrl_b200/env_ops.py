@@ -5,7 +5,8 @@ import ctypes
 import torch
 
 from . import _capi
-from .engine import recompute_adjoint
+from .engine import check_wrench, recompute_adjoint, wrench_struct
+from .modelpack import DfxExternalWrench
 
 
 class DfxWalkerParams(ctypes.Structure):
@@ -73,6 +74,10 @@ def _bind(lib):
     lib.dfx_env_step_backward.argtypes = [V, I, I, I, Dbl, V, V, V, V, ctypes.POINTER(DfxEnvTransitionAdj), V, V, V, V]
     if hasattr(lib, "dfx_env_step_backward_recompute"):
         lib.dfx_env_step_backward_recompute.argtypes = [V, I, I, I, Dbl, V, V, V, V, V, V, ctypes.POINTER(DfxEnvTransitionAdj), V, V, V, V]
+    if hasattr(lib, "dfx_env_step_forward_ex"):
+        W = ctypes.POINTER(DfxExternalWrench)
+        for name in ("dfx_env_step_forward", "dfx_env_step_backward", "dfx_env_step_backward_recompute"):
+            getattr(lib, name + "_ex").argtypes = getattr(lib, name).argtypes + [W]
     lib._walker_bound = True
 
 
@@ -231,10 +236,11 @@ class EnvStepFunction(torch.autograd.Function):
     values bit for bit.  ``amap`` = (offset, pre_scale, pre_bias, drive_scale, strength, is_muscle); ``params`` a
     ``DfxWalkerParams`` or ``DfxPlanarParams``; ``progress`` the counter before the step; ``start_q`` / ``start_qd`` the state a
     terminated environment restarts from (constants for autograd); ``nan_guard``: non-finite input cotangents become 0 (the
-    reference's gradient hooks on the state and the clipped actions, envs/humanoid.py:196-206)."""
+    reference's gradient hooks on the state and the clipped actions, envs/humanoid.py:196-206; the wrench's too).  ``f_ext``:
+    optional external link wrenches [N, L, 6] (``engine.check_wrench``); its gradient is returned when it requires one."""
 
     @staticmethod
-    def forward(ctx, engine, substeps, mm_freq, dt, amap, params, nan_guard, progress, start_q, start_qd, q, qd, raw):
+    def forward(ctx, engine, substeps, mm_freq, dt, amap, params, nan_guard, progress, start_q, start_qd, q, qd, raw, f_ext=None):
         from .modelpack import DfxActionMap
         lib = engine.lib
         _bind(lib)
@@ -242,11 +248,12 @@ class EnvStepFunction(torch.autograd.Function):
         dev = engine.device
         q, qd, raw = _c(q.detach()), _c(qd.detach()), _c(raw.detach())
         start_q, start_qd = _c(start_q), _c(start_qd)
+        f_ext = check_wrench(engine, f_ext)
         n, A = engine.N, raw.shape[-1]
         m = DfxActionMap(int(A), int(offset), int(bool(is_muscle)), float(pre_scale), float(pre_bias), float(drive_scale), strength.data_ptr())
         f32 = dict(dtype=torch.float32, device=dev)
         q_sim, qd_sim, used = torch.empty_like(q), torch.empty_like(qd), torch.empty_like(raw)
-        need = any(ctx.needs_input_grad[10:13])
+        need = any(ctx.needs_input_grad[10:14])
         ctx.nan_guard = nan_guard
         ctx.recompute = recompute_adjoint()
         tape = torch.empty(engine.tape_floats(substeps, mm_freq), **f32) if (need and not ctx.recompute) else None
@@ -266,22 +273,26 @@ class EnvStepFunction(torch.autograd.Function):
                         ("reset", reset), ("q_next", q_next), ("qd_next", qd_next), ("actions_next", actions_next),
                         ("progress_next", progress_next), ("obs_next", obs_next)):
             setattr(tr, name, t.data_ptr())
+        args = (engine.pack, n, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd), ctypes.byref(m), _ptr(raw), None, _ptr(used),
+                _ptr(q_sim), _ptr(qd_sim), _ptr(tape), ctypes.byref(tr), _stream(dev))
         with torch.cuda.device(dev):
-            code = lib.dfx_env_step_forward(engine.pack, n, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd), ctypes.byref(m),
-                                            _ptr(raw), None, _ptr(used), _ptr(q_sim), _ptr(qd_sim), _ptr(tape), ctypes.byref(tr), _stream(dev))
+            if f_ext is None:
+                code = lib.dfx_env_step_forward(*args)
+            else:
+                code = lib.dfx_env_step_forward_ex(*args, wrench_struct(f_ext))
         _capi.check(code, "dfx_env_step_forward")
         ctx.engine, ctx.cfg, ctx.amap, ctx.params = engine, (substeps, mm_freq, dt), m, params
         ctx.strength = strength                      # keeps the device array the struct points at alive
         ctx.set_materialize_grads(False)             # absent cotangents arrive as None (NULL in the C ABI), not as zero fills
         ctx.shapes = (q.shape, qd.shape)
         # recompute mode: the env-step's input state in place of its tape
-        ctx.save_for_backward(raw, tape, q_sim, qd_sim, used, reset, *((q, qd) if ctx.recompute else (None, None)))
+        ctx.save_for_backward(raw, tape, q_sim, qd_sim, used, reset, f_ext, *((q, qd) if ctx.recompute else (None, None)))
         ctx.mark_non_differentiable(reset, progress_next)
         return obs_before, rew, reset, q_next, qd_next, actions_next, progress_next, obs_next
 
     @staticmethod
     def backward(ctx, g_obs_before, g_rew, g_reset, g_q_next, g_qd_next, g_actions_next, g_progress, g_obs_next):
-        raw, tape, q_sim, qd_sim, used, reset, q, qd = ctx.saved_tensors
+        raw, tape, q_sim, qd_sim, used, reset, f_ext, q, qd = ctx.saved_tensors
         engine, (substeps, mm_freq, dt), params = ctx.engine, ctx.cfg, ctx.params
         lib, dev = engine.lib, engine.device
         cot = [None if g is None else _c(g) for g in (g_obs_before, g_rew, g_q_next, g_qd_next, g_actions_next, g_obs_next)]
@@ -300,19 +311,24 @@ class EnvStepFunction(torch.autograd.Function):
         gq = torch.empty(engine.N * engine.Q, dtype=torch.float32, device=dev)
         gqd = torch.empty(engine.N * engine.D, dtype=torch.float32, device=dev)
         g_raw = torch.empty_like(raw)
+        g_f_ext = engine._wrench_grad(f_ext, ctx.needs_input_grad[13] if f_ext is not None else False)
+        ws = wrench_struct(f_ext, g_f_ext)
         if ctx.recompute:
             workspace = engine.recompute_workspace(substeps, mm_freq)
+            args = (engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd), ctypes.byref(ctx.amap), _ptr(raw), None,
+                    _ptr(workspace), ctypes.byref(tr), _ptr(gq), _ptr(gqd), _ptr(g_raw), _stream(dev))
             with torch.cuda.device(dev):
-                code = lib.dfx_env_step_backward_recompute(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), _ptr(q), _ptr(qd),
-                                                           ctypes.byref(ctx.amap), _ptr(raw), None, _ptr(workspace), ctypes.byref(tr),
-                                                           _ptr(gq), _ptr(gqd), _ptr(g_raw), _stream(dev))
+                code = lib.dfx_env_step_backward_recompute(*args) if ws is None else lib.dfx_env_step_backward_recompute_ex(*args, ws)
             _capi.check(code, "dfx_env_step_backward_recompute")
         else:
+            args = (engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), ctypes.byref(ctx.amap), _ptr(raw), None, _ptr(tape),
+                    ctypes.byref(tr), _ptr(gq), _ptr(gqd), _ptr(g_raw), _stream(dev))
             with torch.cuda.device(dev):
-                code = lib.dfx_env_step_backward(engine.pack, engine.N, int(substeps), int(mm_freq), float(dt), ctypes.byref(ctx.amap), _ptr(raw),
-                                                 None, _ptr(tape), ctypes.byref(tr), _ptr(gq), _ptr(gqd), _ptr(g_raw), _stream(dev))
+                code = lib.dfx_env_step_backward(*args) if ws is None else lib.dfx_env_step_backward_ex(*args, ws)
             _capi.check(code, "dfx_env_step_backward")
         if ctx.nan_guard:
-            for g in (gq, gqd, g_raw):
-                torch.nan_to_num(g, nan=0.0, posinf=0.0, neginf=0.0, out=g)
-        return None, None, None, None, None, None, None, None, None, None, gq.view(ctx.shapes[0]), gqd.view(ctx.shapes[1]), g_raw
+            for g in (gq, gqd, g_raw, g_f_ext):
+                if g is not None:
+                    torch.nan_to_num(g, nan=0.0, posinf=0.0, neginf=0.0, out=g)
+        return (None, None, None, None, None, None, None, None, None, None, gq.view(ctx.shapes[0]), gqd.view(ctx.shapes[1]), g_raw,
+                g_f_ext)

@@ -118,6 +118,7 @@ class DFlexEnv:
                 t.register_hook(hook)
 
     nan_guard = False
+    external_wrench = None     # set_external_wrench
     clone_actions = True
     # True: terminated environments are re-initialised with a mask (torch.where) instead of the reference's
     # reset_buf.nonzero() + indexed writes, so env.step() never synchronises the host with the GPU.
@@ -129,6 +130,28 @@ class DFlexEnv:
     # _backward): env.step() is ONE launch forward and ONE backward
     single_launch_step = True
 
+    def set_external_wrench(self, w):
+        """External wrenches on the links, applied on every following step until changed: ``w`` [num_envs, L, 6] fp32 on the
+        env's device -- per link (torque, force), both in world axes, the force applied at the link's centre of mass (MuJoCo's
+        ``xfrc_applied`` convention; include/dfx.h DfxExternalWrench) -- or None for none.  Differentiable: a ``w`` that
+        requires grad receives the gradient of whatever the rollout's loss is.  ``GraphedRollout`` refuses an env with a
+        wrench set."""
+        if w is not None:
+            from ..dflex_api.sim import _engine_for
+            from ..engine import check_wrench
+            engine = _engine_for(self.model)
+            if tuple(w.shape) != (self.num_envs, engine.L, 6):
+                raise ValueError("external wrench has shape %s, expected [%d, %d, 6]" % (tuple(w.shape), self.num_envs, engine.L))
+            check_wrench(engine, w)
+        self.external_wrench = w
+
+    def _attach_wrench(self, state):
+        """The step reads the wrench from its input State (``body_f_ext``)."""
+        if self.external_wrench is None:
+            state.__dict__.pop("body_f_ext", None)
+        else:
+            state.body_f_ext = self.external_wrench
+
     def step(self, actions):
         actions = actions.view((self.num_envs, self.num_actions))
         actions = self._preprocess_actions(torch.clip(actions, -1.0, 1.0))
@@ -136,6 +159,7 @@ class DFlexEnv:
             self._nan_guard(actions)
         self.actions = actions.clone() if self.clone_actions else actions
         self._apply_actions(actions)
+        self._attach_wrench(self.state)
         self.state = self.integrator.forward(self.model, self.state, self.sim_dt, self.sim_substeps, self.MM_caching_frequency)
         self.sim_time += self.sim_dt
         self.reset_buf = torch.zeros_like(self.reset_buf)
@@ -167,6 +191,7 @@ class DFlexEnv:
             self._amap = self._action_map()
             self._tparams = self._transition_params()
         width, offset, pre_scale, pre_bias, drive_scale, strength, is_muscle = self._amap
+        self._attach_wrench(self.state)
         if self.single_launch_step and self.fused_action_map and not self.no_grad:
             from ..dflex_api.sim import fused_env_step
             start_q, start_qd = self._start_state()

@@ -40,6 +40,12 @@ class DfxActionMap(ctypes.Structure):
                 ("strength", ctypes.c_void_p)]
 
 
+class DfxExternalWrench(ctypes.Structure):
+    """include/dfx.h DfxExternalWrench: per-environment link wrenches [N, L, 6] (torque, force at the centre of mass; world
+    axes) for the _ex step entries, and where the adjoint writes their cotangent (NULL: skip)."""
+    _fields_ = [("f_ext", ctypes.c_void_p), ("g_f_ext", ctypes.c_void_p)]
+
+
 class DfxDerived(ctypes.Structure):
     """ctypes mirror of ``DfxDerived`` in include/dfx.h."""
 

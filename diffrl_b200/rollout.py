@@ -26,6 +26,8 @@ class GraphedRollout:
             raise RuntimeError("GraphedRollout needs a CUDA environment")
         if env.no_grad:
             raise RuntimeError("GraphedRollout differentiates the rollout: construct the env with no_grad=False")
+        if getattr(env, "external_wrench", None) is not None:
+            raise RuntimeError("GraphedRollout does not capture external wrenches: call env.set_external_wrench(None) first")
         if not getattr(env, "sync_free_reset", False) or not hasattr(env, "_start_state"):
             raise RuntimeError("%s resets through reset_buf.nonzero(), which cannot be captured" % type(env).__name__)
         self.env, self.T = env, int(horizon)

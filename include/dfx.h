@@ -30,6 +30,20 @@
 extern "C" {
 #endif
 
+/* External wrench on the links, per environment (the _ex twins of the step entries below; a NULL DfxExternalWrench* is no
+ * wrench, and those calls run exactly the code of the entries without _ex).  f_ext [N, L, 6], device, fp32: row (e, i) is
+ * (tau, F), angular part first as in dflex spatial vectors -- F a force in world axes applied AT LINK i's CENTRE OF MASS,
+ * tau a pure torque in world axes (the convention of MuJoCo's xfrc_applied).  It is held constant over the env-step's
+ * substeps, as the actuation.  In the step it enters where gravity does:  body_f_s = f_b - (c x (m g + F) + tau, m g + F),
+ * c = the link's centre of mass.  The backward entries take the SAME f_ext as the forward call and overwrite g_f_ext
+ * [N, L, 6] (NULL: skip) with its cotangent; f_ext == NULL with a non-NULL struct is cudaErrorInvalidValue.  The external-
+ * wrench kernels keep 6 L (forward) / 12 L (backward) more floats of scratch per environment: dfx_launch_plan(pack, 2 | bwd,
+ * ...) tells whether they still fit.  Flag bit 6 (64) of dfx_set_flags has no external-wrench kernels (cudaErrorNotSupported). */
+typedef struct DfxExternalWrench {
+    const float* f_ext;
+    float* g_f_ext;
+} DfxExternalWrench;
+
 /* Static description of ONE articulation (HOST pointers; copied during dfx_pack_create).
  * Field names and layouts are those of the reference Model (dflex/dflex/model.py:1646-1879,
  * collide() :424-515) restricted to a single environment, with link / shape indices made
@@ -143,6 +157,15 @@ int dfx_step_backward(const dfx_pack_t* pack, int num_envs, int substeps, int mm
                       const float* act, const float* musc, const float* tape,
                       const float* gq_out, const float* gqd_out,
                       float* gq, float* gqd, float* gact, float* gmusc, void* stream);
+/* the two above with an external wrench (DfxExternalWrench; NULL: none) */
+int dfx_step_forward_ex(const dfx_pack_t* pack, int num_envs, int substeps, int mm_freq, double dt,
+                        const float* q, const float* qd, const float* act, const float* musc,
+                        float* q_out, float* qd_out, float* tape, const DfxDerived* derived,
+                        void* stream, const DfxExternalWrench* wrench);
+int dfx_step_backward_ex(const dfx_pack_t* pack, int num_envs, int substeps, int mm_freq, double dt,
+                         const float* act, const float* musc, const float* tape,
+                         const float* gq_out, const float* gqd_out,
+                         float* gq, float* gqd, float* gact, float* gmusc, void* stream, const DfxExternalWrench* wrench);
 
 /* ---- fused env epilogue (SURVEY.md section 8f-1): observation + reward + termination flags of the free-root
  * walker envs and its adjoint, replacing ~35 PyTorch ops per env.step (reference envs/ant.py:266-307,
@@ -236,6 +259,13 @@ int dfx_step_backward_mapped(const dfx_pack_t* pack, int n, int substeps, int mm
                              const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
                              const float* gq_out, const float* gqd_out, const float* g_used,
                              float* gq, float* gqd, float* g_raw, void* stream);
+int dfx_step_forward_mapped_ex(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
+                               const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                               float* used, float* q_out, float* qd_out, float* tape, void* stream, const DfxExternalWrench* wrench);
+int dfx_step_backward_mapped_ex(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
+                                const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
+                                const float* gq_out, const float* gqd_out, const float* g_used,
+                                float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* wrench);
 
 /* ---- env.step() as ONE launch (SURVEY.md section 8f-1: "fuse into the step epilogue (and its adjoint)"; reference
  * envs/ant.py:156-190 = the action map, SemiImplicitIntegrator.forward and the transition, ~40 PyTorch kernels + one per
@@ -266,6 +296,10 @@ typedef struct DfxEnvTransition {
 int dfx_env_step_forward(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
                          const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                          float* used, float* q_sim, float* qd_sim, float* tape, const DfxEnvTransition* tr, void* stream);
+int dfx_env_step_forward_ex(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
+                            const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                            float* used, float* q_sim, float* qd_sim, float* tape, const DfxEnvTransition* tr, void* stream,
+                            const DfxExternalWrench* wrench);
 typedef struct DfxEnvTransitionAdj {
     int kind;
     DfxWalkerParams walker;
@@ -288,6 +322,9 @@ typedef struct DfxEnvTransitionAdj {
 int dfx_env_step_backward(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
                           const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
                           const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream);
+int dfx_env_step_backward_ex(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
+                             const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
+                             const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* wrench);
 
 /* ---- recompute adjoint: backward WITHOUT a stored tape.  The forward then runs with tape == NULL (the no-grad launch) and
  * keeps nothing; each adjoint entry below re-runs the env-step's forward from its input state (q, qd) and actuation into a
@@ -316,6 +353,19 @@ int dfx_step_backward_mapped_recompute(const dfx_pack_t* pack, int n, int subste
 int dfx_env_step_backward_recompute(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
                                     const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                                     float* workspace, const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream);
+/* the three recompute entries with an external wrench (DfxExternalWrench: the f_ext of the forward call; NULL: none) */
+int dfx_step_backward_recompute_ex(const dfx_pack_t* pack, int num_envs, int substeps, int mm_freq, double dt,
+                                   const float* q, const float* qd, const float* act, const float* musc, float* workspace,
+                                   const float* gq_out, const float* gqd_out,
+                                   float* gq, float* gqd, float* gact, float* gmusc, void* stream, const DfxExternalWrench* wrench);
+int dfx_step_backward_mapped_recompute_ex(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
+                                          const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                                          float* workspace, const float* gq_out, const float* gqd_out, const float* g_used,
+                                          float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* wrench);
+int dfx_env_step_backward_recompute_ex(const dfx_pack_t* pack, int n, int substeps, int mm_freq, double dt,
+                                       const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
+                                       float* workspace, const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream,
+                                       const DfxExternalWrench* wrench);
 
 /* Launch configuration knob: lanes cooperating on one environment (8, 16 or 32; 0 = auto). */
 int dfx_set_group_size(int lanes);
@@ -338,7 +388,8 @@ int dfx_set_tape_dtype(int bf16);
  * (32 environments per CTA for Ant / Hopper / HalfCheetah / CartPole, 8 for the two humanoids); 8, 16 or 32 = only a
  * kernel of that width (an articulation without one falls back to the lane-group kernels).  For A/B timing and tests. */
 int dfx_set_tile_envs(int envs);
-/* Launch geometry the step kernel would use for this pack (host arithmetic, no GPU needed):
+/* Launch geometry the step kernel would use for this pack (host arithmetic, no GPU needed); `backward`: bit 0 the adjoint,
+ * bit 1 (2) the external-wrench kernels (DfxExternalWrench).  out[1] == 0: that kernel does not fit one CTA's shared memory.
  * out[0] lanes per environment, out[1] environments per CTA, out[2] CTAs per SM (shared-memory / register bound),
  * out[3] dynamic shared memory per CTA in bytes, out[4] scratch floats per environment, out[5] bytes of the staged pack + CTA task list. */
 int dfx_launch_plan(const dfx_pack_t* pack, int backward, int out[6]);
@@ -346,7 +397,8 @@ int dfx_launch_plan(const dfx_pack_t* pack, int backward, int out[6]);
 long long dfx_launch_count(void);
 const char* dfx_version(void);
 /* sizeof() of the parameter structs as THIS library was compiled (a binding's struct mirrors can check themselves against it):
- * 0 DfxModelDesc, 1 DfxDerived, 2 DfxWalkerParams, 3 DfxPlanarParams, 4 DfxActionMap, 5 DfxEnvTransition, 6 DfxEnvTransitionAdj;
+ * 0 DfxModelDesc, 1 DfxDerived, 2 DfxWalkerParams, 3 DfxPlanarParams, 4 DfxActionMap, 5 DfxEnvTransition, 6 DfxEnvTransitionAdj,
+ * 7 DfxExternalWrench;
  * anything else: -1. */
 int dfx_abi_sizeof(int which);
 /* Joint types the size-specialised tile kernels of an articulation with these sizes are COMPILED for (a bit mask as in
