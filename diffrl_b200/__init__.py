@@ -1,3 +1,4 @@
+import collections
 
 
 def set_tape_dtype(dtype="fp32"):
@@ -29,3 +30,25 @@ def set_adjoint_mode(mode="tape"):
     if mode == "recompute" and not hasattr(_capi.lib(), "dfx_step_backward_recompute"):
         raise _capi.DfxError("%s has no recompute adjoint (dfx_step_backward_recompute): rebuild it" % _capi.LIB_PATH)
     engine.adjoint_mode = mode
+
+
+def link_state(model, joint_q, joint_qd):
+    """The pose and velocity of every link of the state (joint_q, joint_qd) of ``model``'s N environments, differentiable:
+    ``LinkState(body_X_sc, body_X_sm, body_v_s)`` in the layouts of the reference State fields --
+
+    - ``body_X_sc`` [N, L, 7]: the link frame in world, position then quaternion xyzw;
+    - ``body_X_sm`` [N, L, 7]: the centre-of-mass frame X_sc * X_cm (its position is where an external wrench applies its force);
+    - ``body_v_s`` [N, L, 6]: the spatial twist (w, v_o) in world axes, v_o the velocity of the body-fixed point at the world
+      origin; the centre of mass moves with ``v_o + w x X_sm.p``.
+
+    One kernel launch forward (include/dfx.h dfx_link_state_forward) and one backward, which recomputes the kinematics from
+    (joint_q, joint_qd) -- nothing is kept but the inputs, in either adjoint mode.  joint_q [N*Q] or [N, Q], joint_qd [N*D] or
+    [N, D], fp32 on the model's device (ValueError otherwise); quaternions are used as given, not renormalised.  Unlike the
+    State's derived fields (the start of the last substep of the step that produced a State, no gradient), this is the state
+    given, and gradients flow into it."""
+    from .dflex_api.sim import _engine_for
+    from .engine import LinkStateFunction
+    return LinkState(*LinkStateFunction.apply(_engine_for(model), joint_q, joint_qd))
+
+
+LinkState = collections.namedtuple("LinkState", ["body_X_sc", "body_X_sm", "body_v_s"])

@@ -69,6 +69,9 @@ def lib():
         for name in ("dfx_step_forward", "dfx_step_backward", "dfx_step_forward_mapped", "dfx_step_backward_mapped",
                      "dfx_step_backward_recompute", "dfx_step_backward_mapped_recompute"):
             getattr(L, name + "_ex").argtypes = getattr(L, name).argtypes + [W]
+    if hasattr(L, "dfx_link_state_forward"):    # link state of (q, qd) (include/dfx.h dfx_link_state_*)
+        L.dfx_link_state_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, ctypes.c_void_p]
+        L.dfx_link_state_backward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, _F, _F, ctypes.c_void_p]
     if os.environ.get("DFX_FLAGS"):      # tuning flags of include/dfx.h (A/B runs of the test-suite)
         L.dfx_set_flags(int(os.environ["DFX_FLAGS"]))
     _lib = L

@@ -206,6 +206,45 @@ __global__ void __launch_bounds__(kMaxThreads) dfx_step_wrench_kernel(const __gr
     step_kernel_body<G, BACKWARD, SL, SD, SQ, SC, SM, true>(ka);
 }
 
+// Link state (include/dfx.h dfx_link_state_forward / _backward; dfx_step.h link_state_*): the set-up of step_kernel_body, then the
+// kinematics of (q, qd) or their adjoint in the step's forward / backward layout.  The pointers come as a kernel parameter of their
+// own (KernelArgs stays as the step kernels have it).
+template <int G, bool BACKWARD, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(kMaxThreads) dfx_link_state_kernel(const __grid_constant__ KernelArgs ka,
+                                                                    const __grid_constant__ LinkStateArgs la) {
+    extern __shared__ __align__(16) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += blockDim.x) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += blockDim.x) ipack[i] = ka.blob.ints[i];
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    Layout Y = ka.layout;
+    if constexpr (SL > 0) {
+        P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+        constexpr Layout kY = make_layout(SL, SD, SQ, SC, SM);
+        Y = kY;
+    }
+    const int kEnvsPerCta = blockDim.x / G;
+    const int local = threadIdx.x / G;
+    int env = blockIdx.x * kEnvsPerCta + local;      // (groups past the end redo the last environment, as in step_kernel_body)
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const int lane_in_warp = threadIdx.x & 31;
+    GroupCuda<G> g;
+    g.lane = threadIdx.x % G;
+    g.psync = (ka.step.flags & 2) != 0;
+    g.mask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << ((lane_in_warp / G) * G));
+    float* s = smem + ka.pack_smem_floats + ka.cta_area_floats + (size_t)local * ka.scratch_stride;
+    g.scratch0 = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    g.task_count = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    g.task_list = g.task_count + 4;
+    g.stride = ka.scratch_stride;
+    g.envs_shift = 31 - __clz(kEnvsPerCta > 0 ? kEnvsPerCta : 1);
+    g.cta_mode = (ka.step.flags & 8) != 0;
+    if (BACKWARD) link_state_backward(P, Y, s, g, env, la);
+    else link_state_forward(P, Y, s, g, env, la);
+}
+
 }  // namespace dfx
 
 // =====================================================================================
@@ -415,6 +454,16 @@ static cudaError_t launch_impl(const dfx_pack* p, const StepArgs& step, const Df
     return cudaGetLastError();
 }
 
+// the size-specialised lane-group instantiations (the six DiffRL articulations), by the group width pick_group() chooses for them
+#define DFX_GROUP_SPECIALS_16(X)                                                                     \
+    X(9, 14, 15, 25, 0)      /* Ant */                                                               \
+    X(3, 2, 2, 0, 0)         /* CartPole */                                                          \
+    X(6, 6, 6, 8, 0)         /* Hopper */                                                            \
+    X(9, 9, 9, 16, 0)        /* HalfCheetah */
+#define DFX_GROUP_SPECIALS_32(X)                                                                     \
+    X(22, 27, 28, 35, 0)     /* Humanoid */                                                          \
+    X(11, 24, 29, 88, 152)   /* SNU humanoid (lower body, 152 muscles) */
+
 // dispatch on the model sizes: specialised instantiations for the DiffRL articulations, generic otherwise
 template <int G, bool BWD, bool WRENCH>
 static cudaError_t launch(const dfx_pack* p, const StepArgs& step, const DfxExternalWrench& w, cudaStream_t stream) {
@@ -422,19 +471,48 @@ static cudaError_t launch(const dfx_pack* p, const StepArgs& step, const DfxExte
 #define DFX_SPECIAL(l, d, q, c, m) \
     if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return launch_impl<G, BWD, WRENCH, l, d, q, c, m>(p, step, w, stream);
     if (!(g_flags & 4)) {
-        if constexpr (G == 16) {               // the group width pick_group() chooses for these models
-            DFX_SPECIAL(9, 14, 15, 25, 0)      // Ant
-            DFX_SPECIAL(3, 2, 2, 0, 0)         // CartPole
-            DFX_SPECIAL(6, 6, 6, 8, 0)         // Hopper
-            DFX_SPECIAL(9, 9, 9, 16, 0)        // HalfCheetah
-        }
-        if constexpr (G == 32) {
-            DFX_SPECIAL(22, 27, 28, 35, 0)     // Humanoid
-            DFX_SPECIAL(11, 24, 29, 88, 152)   // SNU humanoid (lower body, 152 muscles)
-        }
+        if constexpr (G == 16) { DFX_GROUP_SPECIALS_16(DFX_SPECIAL) }
+        if constexpr (G == 32) { DFX_GROUP_SPECIALS_32(DFX_SPECIAL) }
     }
 #undef DFX_SPECIAL
     return launch_impl<G, BWD, WRENCH, 0, 0, 0, 0, 0>(p, step, w, stream);
+}
+
+// the link state (dfx_link_state_kernel) with the step kernel's launch geometry for the same pass
+template <int G, bool BWD, int SL, int SD, int SQ, int SC, int SM>
+static cudaError_t link_state_launch_impl(const dfx_pack* p, int n, const LinkStateArgs& la, cudaStream_t stream) {
+    KernelArgs ka;
+    memset(&ka, 0, sizeof ka);
+    ka.header = p->header;
+    ka.blob = p->blob;
+    ka.layout = BWD ? p->host.layout_bwd : p->host.layout;
+    ka.step.N = n;
+    ka.step.flags = g_flags;
+    const LaunchPlan lp = plan_launch(p, G, BWD);
+    ka.scratch_stride = lp.scratch_stride;
+    ka.pack_smem_floats = lp.pack_bytes / 4;
+    ka.cta_area_floats = lp.cta_area_bytes / 4;
+    if (lp.envs_per_cta == 0) return cudaErrorInvalidConfiguration;
+    auto kern = dfx_link_state_kernel<G, BWD, SL, SD, SQ, SC, SM>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lp.smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (n + lp.envs_per_cta - 1) / lp.envs_per_cta;
+    kern<<<grid, lp.envs_per_cta * G, lp.smem, stream>>>(ka, la);
+    g_launches.fetch_add(1);
+    return cudaGetLastError();
+}
+
+template <int G, bool BWD>
+static cudaError_t launch_link_state(const dfx_pack* p, int n, const LinkStateArgs& la, cudaStream_t stream) {
+    const Pack& h = p->header;
+#define DFX_SPECIAL(l, d, q, c, m) \
+    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return link_state_launch_impl<G, BWD, l, d, q, c, m>(p, n, la, stream);
+    if (!(g_flags & 4)) {
+        if constexpr (G == 16) { DFX_GROUP_SPECIALS_16(DFX_SPECIAL) }
+        if constexpr (G == 32) { DFX_GROUP_SPECIALS_32(DFX_SPECIAL) }
+    }
+#undef DFX_SPECIAL
+    return link_state_launch_impl<G, BWD, 0, 0, 0, 0, 0>(p, n, la, stream);
 }
 
 static cudaError_t launch_tile(const dfx_pack* p, const StepArgs& step, bool backward, const DfxExternalWrench* w, cudaStream_t stream) {
@@ -835,6 +913,55 @@ int dfx_env_step_backward_recompute_ex(const dfx_pack_t* p, int n, int substeps,
     a.env_kind = tr->kind;
     a.env_adj = *tr;
     return run_recompute_fused(p, a, q, qd, workspace, stream, w);
+}
+
+// ---- link state (include/dfx.h dfx_link_state_*): the kernel family the step entries pick for the pack -- its tile kernels, or
+// the lane-group kernels of pick_group()'s width, generic under flag bit 2 (4).  The flag-64 A/B variants run the default tile
+// kernels (no tape layout to match).
+static int run_link_state(const dfx_pack_t* p, int n, const LinkStateArgs& la, bool backward, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (p->tile) {
+        KernelArgs ka;
+        memset(&ka, 0, sizeof ka);
+        ka.header = p->header;
+        ka.blob = p->blob;
+        ka.step.N = n;
+        ka.step.flags = g_flags;
+        int e = (int)cudaErrorInvalidConfiguration;
+        switch (p->tile) {
+            case 8: e = dfx_tile_launch_link_state_e8(&ka, &la, backward, stream); break;
+            case 16: e = dfx_tile_launch_link_state_e16(&ka, &la, backward, stream); break;
+            case 32: e = dfx_tile_launch_link_state_e32(&ka, &la, backward, stream); break;
+        }
+        g_launches.fetch_add(1);
+        return e;
+    }
+    switch (pick_group(p)) {
+        case 8: return (int)(backward ? launch_link_state<8, true>(p, n, la, st) : launch_link_state<8, false>(p, n, la, st));
+        case 16: return (int)(backward ? launch_link_state<16, true>(p, n, la, st) : launch_link_state<16, false>(p, n, la, st));
+        default: return (int)(backward ? launch_link_state<32, true>(p, n, la, st) : launch_link_state<32, false>(p, n, la, st));
+    }
+}
+
+int dfx_link_state_forward(const dfx_pack_t* p, int n, const float* q, const float* qd,
+                           float* body_X_sc, float* body_X_sm, float* body_v_s, void* stream) {
+    if (!p || n <= 0 || !q || !qd) return (int)cudaErrorInvalidValue;
+    if (!body_X_sc && !body_X_sm && !body_v_s) return 0;
+    LinkStateArgs la;
+    memset(&la, 0, sizeof la);
+    la.q = q; la.qd = qd; la.X_sc = body_X_sc; la.X_sm = body_X_sm; la.v_s = body_v_s;
+    return run_link_state(p, n, la, false, stream);
+}
+
+int dfx_link_state_backward(const dfx_pack_t* p, int n, const float* q, const float* qd,
+                            const float* g_X_sc, const float* g_X_sm, const float* g_v_s,
+                            float* gq, float* gqd, void* stream) {
+    if (!p || n <= 0 || !q || !qd) return (int)cudaErrorInvalidValue;
+    if (!gq && !gqd) return 0;
+    LinkStateArgs la;
+    memset(&la, 0, sizeof la);
+    la.q = q; la.qd = qd; la.g_X_sc = g_X_sc; la.g_X_sm = g_X_sm; la.g_v_s = g_v_s; la.gq = gq; la.gqd = gqd;
+    return run_link_state(p, n, la, true, stream);
 }
 
 }  // extern "C"

@@ -77,7 +77,9 @@ struct KernelArgs {
     size_t dfx_tile_smem_e##E(const void* kernel_args, int backward);                                                \
     /* wrench != 0: the external-wrench kernels (kernel_args' `wrench`) */                                             \
     int dfx_tile_launch_e##E(void* kernel_args, int backward, int wrench, void* stream);                             \
-    int dfx_tile_launch_recompute_e##E(void* kernel_args, int wrench, void* stream);   /* forward into the workspace + adjoint, one launch */
+    int dfx_tile_launch_recompute_e##E(void* kernel_args, int wrench, void* stream);   /* forward into the workspace + adjoint, one launch */ \
+    /* the link state (link_args: a LinkStateArgs); backward != 0: its adjoint */                                     \
+    int dfx_tile_launch_link_state_e##E(void* kernel_args, const void* link_args, int backward, void* stream);
 DFX_DECLARE_TILE(8)
 DFX_DECLARE_TILE(16)
 DFX_DECLARE_TILE(32)

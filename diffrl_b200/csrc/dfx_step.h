@@ -216,4 +216,61 @@ DFX_HD void env_step_backward(const Pack& P, const Layout& Y, SP s, const Grp& g
     }
 }
 
+// ---- link state of (q, qd) (include/dfx.h dfx_link_state_forward / _backward): the kinematics of one substep on its own --
+// X_sc, X_sm (reference eval_rigid_fk) and v (the velocity half of eval_rigid_id) -- in the step's forward and backward
+// layouts, which hold every field these touch.  The kernels get these pointers as a kernel parameter of their own, next to
+// KernelArgs (whose `step.N` and `step.flags` they read), so KernelArgs / StepArgs stay as the step kernels have them.
+struct LinkStateArgs {
+    const float* q; const float* qd;
+    float* X_sc; float* X_sm; float* v_s;                       // forward outputs [N, L, 7 / 7 / 6] (NULL: skip)
+    const float* g_X_sc; const float* g_X_sm; const float* g_v_s;   // backward: their cotangents (NULL == 0)
+    float* gq; float* gqd;                                      // backward outputs [N, Q], [N, D] (NULL: skip)
+};
+
+// (q, qd) -> X_sc, X_sm, S, v, a in the scratch, as a substep's kinematics (K1 first when the fused phases leave it to
+// integrate_fwd, as env_step_forward does before its first substep)
+template <class Grp>
+DFX_HD void link_state_kinematics(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const LinkStateArgs& a) {
+    DFX_FOR(i, P.Q) s[Y.q + i] = a.q[(long long)env * P.Q + i];
+    DFX_FOR(i, P.D) s[Y.qd + i] = a.qd[(long long)env * P.D + i];
+    g.sync();
+    if constexpr (Grp::kFusedPhases) {
+        DFX_FOR(i, P.L) kin_local_fwd(P, Y, s, i);
+        g.sync();
+    }
+    kin_fwd(P, Y, s, g);
+    g.sync();
+}
+
+template <class Grp>
+DFX_HD void link_state_forward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const LinkStateArgs& a) {
+    const int L = P.L;
+    link_state_kinematics(P, Y, s, g, env, a);
+    if (a.X_sc) DFX_FOR(i, L * 7) a.X_sc[(long long)env * L * 7 + i] = s[Y.Xsc + i];
+    if (a.X_sm) DFX_FOR(i, L * 7) a.X_sm[(long long)env * L * 7 + i] = s[Y.Xsm + i];
+    if (a.v_s) DFX_FOR(i, L * 6) a.v_s[(long long)env * L * 6 + i] = s[Y.v + i];
+}
+
+// adjoint: the kinematics recomputed from (q, qd), the cotangents of X_sc, X_sm, v seeded, nothing downstream (aa, aS zero),
+// then A1 for every link and the rest of the kinematics adjoint, as at the end of substep_adj
+template <class Grp>
+DFX_HD void link_state_backward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const LinkStateArgs& a) {
+    const int L = P.L, Q = P.Q, D = P.D;
+    link_state_kinematics(P, Y, s, g, env, a);
+    DFX_FOR(i, L * 7) s[Y.aXsc + i] = a.g_X_sc ? a.g_X_sc[(long long)env * L * 7 + i] : 0.0f;
+    DFX_FOR(i, L * 7) s[Y.aXsm + i] = a.g_X_sm ? a.g_X_sm[(long long)env * L * 7 + i] : 0.0f;
+    DFX_FOR(i, L * 6) s[Y.av + i] = a.g_v_s ? a.g_v_s[(long long)env * L * 6 + i] : 0.0f;
+    DFX_FOR(i, L * 6) s[Y.aa + i] = 0.0f;
+    DFX_FOR(i, D * 6) s[Y.aS + i] = 0.0f;
+    DFX_FOR(i, Q) s[Y.aq + i] = 0.0f;
+    DFX_FOR(i, D) s[Y.aqd + i] = 0.0f;
+    g.sync();
+    DFX_FOR(i, L) kin_adj_local(P, Y, s, i);
+    g.sync();
+    kin_adj(P, Y, s, g);
+    g.sync();
+    if (a.gq) DFX_FOR(i, Q) a.gq[(long long)env * Q + i] = s[Y.aq + i];
+    if (a.gqd) DFX_FOR(i, D) a.gqd[(long long)env * D + i] = s[Y.aqd + i];
+}
+
 }  // namespace dfx

@@ -406,6 +406,44 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_recompute_wrench_kerne
     tile_recompute_body<NW, PATH, MODE, SL, SD, SQ, SC, SM, true>(ka);
 }
 
+// Link state (include/dfx.h dfx_link_state_forward / _backward; dfx_step.h link_state_*): the kinematics of (q, qd) and their
+// adjoint with the step kernel's group policy (path passes, fused phases) and its forward / backward layout.  No tape, so no
+// mbarriers; the pointers come as a kernel parameter of their own (KernelArgs stays as the step kernels have it).
+template <int NW, int MINB, bool BACKWARD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_link_state_kernel(const __grid_constant__ KernelArgs ka,
+                                                                           const __grid_constant__ LinkStateArgs la) {
+    constexpr int E = DFX_TILE_E;
+    extern __shared__ __align__(128) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += NW * 32) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += NW * 32) ipack[i] = ka.blob.ints[i];
+    int* cta_area = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    if (threadIdx.x < 4) cta_area[threadIdx.x] = 0;
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+    P.jmask = tile_joint_mask(SL, SD, SQ, SC, SM);
+    constexpr Layout Y = make_layout(SL, SD, SQ, SC, SM, MODE, BACKWARD);
+
+    GroupTile<NW, E, PATH> g;
+    const int lane32 = threadIdx.x & 31;
+    g.lane = (threadIdx.x >> 5) * (32 / E) + lane32 / E;
+    g.e = lane32 % E;
+    g.tile = blockIdx.x;
+    g.ntiles = gridDim.x;
+    g.task_count = cta_area;
+    g.task_list = cta_area + 8;
+    g.mbar = nullptr;
+    g.par0 = g.par1 = 0u;
+    g.tile_base = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    int env = blockIdx.x * E + g.e;          // (lanes past the end redo the last environment, as in dfx_tile_kernel)
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const SP s{g.tile_base + g.e};
+    if (BACKWARD) link_state_backward(P, Y, s, g, env, la);
+    else link_state_forward(P, Y, s, g, env, la);
+}
+
 // 128-byte aligned offsets so that the bulk copies of the tile stay 16-byte aligned
 static int tile_pack_floats(const KernelArgs& ka) {
     const int bytes = (((ka.blob.n_floats + 3) & ~3) + ((ka.blob.n_ints + 3) & ~3)) * 4;
@@ -450,6 +488,24 @@ static cudaError_t tile_recompute_launch_impl(KernelArgs& ka, cudaStream_t strea
     if (e != cudaSuccess) return e;
     const int ntiles = (ka.step.N + DFX_TILE_E - 1) / DFX_TILE_E;
     kern<<<ntiles, NW * 32, smem, stream>>>(ka);
+    return cudaGetLastError();
+}
+
+// the step kernel's scratch (same layout, no tape): whatever the step fits, this fits
+template <int NW, int MINB, bool BWD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+static cudaError_t tile_link_state_launch_impl(KernelArgs& ka, const LinkStateArgs& la, cudaStream_t stream) {
+    constexpr Layout Y = make_layout(SL, SD, SQ, SC, SM, MODE, BWD);
+    const int per_env = ((BWD ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
+    ka.layout = Y;
+    ka.pack_smem_floats = tile_pack_floats(ka);
+    ka.cta_area_floats = tile_area_floats(ka);
+    ka.scratch_stride = per_env;
+    const size_t smem = (size_t)(ka.pack_smem_floats + ka.cta_area_floats + per_env * DFX_TILE_E) * sizeof(float);
+    auto kern = dfx_tile_link_state_kernel<NW, MINB, BWD, PATH, MODE, SL, SD, SQ, SC, SM>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int ntiles = (ka.step.N + DFX_TILE_E - 1) / DFX_TILE_E;
+    kern<<<ntiles, NW * 32, smem, stream>>>(ka, la);
     return cudaGetLastError();
 }
 
@@ -554,6 +610,22 @@ int DFX_TILE_FN(dfx_tile_launch_recompute)(void* kargs, int wrench, void* stream
     if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
         return (int)(wrench ? tile_recompute_launch_impl<nwb, minb, path, (mode) & 3, l, d, q, c, m, true>(ka, st)   \
                             : tile_recompute_launch_impl<nwb, minb, path, (mode) & 3, l, d, q, c, m, false>(ka, st));
+    DFX_TILE_MODELS(X)
+#undef X
+    return (int)cudaErrorInvalidConfiguration;
+}
+
+// the link state (dfx_tile_link_state_kernel) of every DFX_TILE_MODELS entry, with the step kernels' warps and occupancy.  The
+// flag-64 (A/B) variants have none: they run these, which is valid because the link state has no tape layout to match.
+int DFX_TILE_FN(dfx_tile_launch_link_state)(void* kargs, const void* largs, int backward, void* stream) {
+    KernelArgs& ka = *static_cast<KernelArgs*>(kargs);
+    const LinkStateArgs& la = *static_cast<const LinkStateArgs*>(largs);
+    const Pack& h = ka.header;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+#define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
+    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
+        return (int)(backward ? tile_link_state_launch_impl<nwb, minb, true, path, (mode) & 3, l, d, q, c, m>(ka, la, st)   \
+                              : tile_link_state_launch_impl<nwf, minb, false, path, (mode) & 3, l, d, q, c, m>(ka, la, st));
     DFX_TILE_MODELS(X)
 #undef X
     return (int)cudaErrorInvalidConfiguration;

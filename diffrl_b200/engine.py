@@ -62,6 +62,26 @@ def check_wrench(engine, f_ext):
     return f_ext.detach().contiguous()
 
 
+def check_link_input(engine, name, t, shapes):
+    """``t``: an input of the link state -- fp32 on the engine's device, of one of ``shapes`` (the state: [N*Q] or [N, Q],
+    [N*D] or [N, D]; the cotangents: the outputs' shapes).  Returns it detached and contiguous (None stays None); anything else
+    is a ValueError, in the style of ``check_wrench``."""
+    if t is None:
+        return None
+    if not isinstance(t, torch.Tensor):
+        raise ValueError("%s must be a torch.Tensor, got %s" % (name, type(t).__name__))
+    if t.dtype != torch.float32:
+        raise ValueError("%s must be float32, got %s" % (name, t.dtype))
+    if t.device != engine.device:
+        raise ValueError("%s is on %s, the engine on %s" % (name, t.device, engine.device))
+    if tuple(t.shape) not in shapes:
+        raise ValueError("%s has shape %s, expected %s" % (name, tuple(t.shape), " or ".join(str(list(s)) for s in shapes)))
+    return t.detach().contiguous()
+
+
+LINK_STATE_FIELDS = ("body_X_sc", "body_X_sm", "body_v_s")
+
+
 def wrench_struct(f_ext, g_f_ext=None):
     """The DfxExternalWrench of an _ex entry (by reference), or None: no wrench."""
     if f_ext is None:
@@ -305,6 +325,42 @@ class ArticulationEngine:
             return gq, gqd, gact, gmusc
         return gq, gqd, gact, gmusc, g_f_ext
 
+    def _link_state_inputs(self, q, qd):
+        if not hasattr(self.lib, "dfx_link_state_forward"):
+            raise _capi.DfxError("%s has no link-state entries (dfx_link_state_*)" % _capi.LIB_PATH)
+        q = check_link_input(self, "q", q, ((self.N * self.Q,), (self.N, self.Q)))
+        qd = check_link_input(self, "qd", qd, ((self.N * self.D,), (self.N, self.D)))
+        return q, qd
+
+    def link_state(self, q, qd, want=LINK_STATE_FIELDS):
+        """(body_X_sc [N, L, 7], body_X_sm [N, L, 7], body_v_s [N, L, 6]) of the state (q, qd) -- ``dfx_link_state_forward``: link
+        frame and centre-of-mass frame in world (position, quaternion xyzw), spatial twist (w, v_o) in world axes; the centre of
+        mass moves with v_o + w x X_sm.p.  The fields not in ``want`` are None (not computed).  q [N*Q] or [N, Q], qd [N*D] or
+        [N, D], fp32 on the engine's device (ValueError otherwise); quaternions are used as given."""
+        q, qd = self._link_state_inputs(q, qd)
+        dev, N, L = self.device, self.N, self.L
+        out = tuple(torch.empty((N, L, 7 if name != "body_v_s" else 6), dtype=torch.float32, device=dev) if name in want else None
+                    for name in LINK_STATE_FIELDS)
+        with torch.cuda.device(dev):
+            code = self.lib.dfx_link_state_forward(self.pack, N, _ptr(q), _ptr(qd), *(_ptr(o) for o in out), self._stream())
+        _capi.check(code, "dfx_link_state_forward")
+        return out
+
+    def link_state_backward(self, q, qd, g_X_sc, g_X_sm, g_v_s, need=(True, True)):
+        """Cotangents (gq [N*Q], gqd [N*D]) of the state from those of (body_X_sc, body_X_sm, body_v_s) (None: zero) --
+        ``dfx_link_state_backward``, which recomputes the kinematics of (q, qd).  An output not in ``need`` is None."""
+        q, qd = self._link_state_inputs(q, qd)
+        N, L = self.N, self.L
+        g = [check_link_input(self, "g_" + name, t, ((N, L, w), (N * L, w), (N * L * w,)))
+             for name, t, w in zip(LINK_STATE_FIELDS, (g_X_sc, g_X_sm, g_v_s), (7, 7, 6))]
+        gq = torch.empty(N * self.Q, dtype=torch.float32, device=self.device) if need[0] else None
+        gqd = torch.empty(N * self.D, dtype=torch.float32, device=self.device) if need[1] else None
+        with torch.cuda.device(self.device):
+            code = self.lib.dfx_link_state_backward(self.pack, N, _ptr(q), _ptr(qd), *(_ptr(x) for x in g), _ptr(gq), _ptr(gqd),
+                                                    self._stream())
+        _capi.check(code, "dfx_link_state_backward")
+        return gq, gqd
+
 
 class MappedSimStepFunction(torch.autograd.Function):
     """(q, qd, raw policy output) -> (q', qd', used): the env-step with the action map folded into the simulation launch
@@ -381,6 +437,29 @@ class MappedSimStepFunction(torch.autograd.Function):
                     code = engine.lib.dfx_step_backward_mapped_ex(*args, wrench_struct(f_ext, g_f_ext))
             _capi.check(code, "dfx_step_backward_mapped")
         return None, None, None, None, None, gq.view(ctx.shapes[0]), gqd.view(ctx.shapes[1]), g_raw, g_f_ext
+
+
+class LinkStateFunction(torch.autograd.Function):
+    """(q, qd) -> (body_X_sc [N, L, 7], body_X_sm [N, L, 7], body_v_s [N, L, 6]): the pose and velocity of every link
+    (``ArticulationEngine.link_state``; the centre of mass moves with v_o + w x X_sm.p).  Saves only (q, qd): the backward
+    recomputes the kinematics, so it is the same in "tape" and "recompute" adjoint mode."""
+
+    @staticmethod
+    def forward(ctx, engine, q, qd):
+        qc, qdc = engine._link_state_inputs(q, qd)
+        out = engine.link_state(qc, qdc)
+        ctx.engine, ctx.shapes = engine, (q.shape, qd.shape)
+        ctx.set_materialize_grads(False)      # a missing cotangent is NULL for dfx_link_state_backward, not a zero fill
+        ctx.save_for_backward(qc, qdc)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_X_sc, g_X_sm, g_v_s):
+        q, qd = ctx.saved_tensors
+        dev = ctx.engine.device
+        g = [None if x is None else _f32c(x, dev) for x in (g_X_sc, g_X_sm, g_v_s)]
+        gq, gqd = ctx.engine.link_state_backward(q, qd, *g, need=tuple(ctx.needs_input_grad[1:3]))
+        return None, None if gq is None else gq.view(ctx.shapes[0]), None if gqd is None else gqd.view(ctx.shapes[1])
 
 
 class SimStepFunction(torch.autograd.Function):

@@ -145,6 +145,13 @@ class DFlexEnv:
             check_wrench(engine, w)
         self.external_wrench = w
 
+    def link_state(self):
+        """``diffrl_b200.link_state`` of ``self.state``, the state the next step starts from: ``LinkState(body_X_sc, body_X_sm,
+        body_v_s)``, [num_envs, L, 7 / 7 / 6].  Differentiable: its gradient reaches the actions and the start state through
+        whichever step op produced ``self.state``."""
+        from .. import link_state
+        return link_state(self.model, self.state.joint_q, self.state.joint_qd)
+
     def _attach_wrench(self, state):
         """The step reads the wrench from its input State (``body_f_ext``)."""
         if self.external_wrench is None:

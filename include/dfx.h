@@ -367,6 +367,24 @@ int dfx_env_step_backward_recompute_ex(const dfx_pack_t* pack, int n, int subste
                                        float* workspace, const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream,
                                        const DfxExternalWrench* wrench);
 
+/* ---- link state: the pose and velocity of every link of (q, qd), differentiable -- the kinematics of one substep on its own
+ * (reference eval_rigid_fk sim.py:1681 and the velocity half of eval_rigid_id sim.py:1845), in the layouts of the reference State
+ * fields (model.py:360-388):
+ *   body_X_sc [n*L*7]  link frame in world: position, quaternion xyzw;
+ *   body_X_sm [n*L*7]  centre-of-mass frame X_sc * X_cm (its position is where DfxExternalWrench applies the force);
+ *   body_v_s  [n*L*6]  spatial twist (w, v_o) in world axes, v_o the velocity of the body-fixed point at the world origin:
+ *                      the centre of mass moves with v_o + w x X_sm.p.
+ * Quaternions in q are used as given (not renormalised), so the adjoint has the component along |q|, as the step's.  The backward
+ * recomputes the kinematics from (q, qd) and keeps nothing between the calls.  Both run on the kernel family the step entries use
+ * for the pack, in the step's scratch layouts: an articulation the step fits, these fit.  Stream-ordered, no host synchronisation. */
+/* link poses / velocities of (q, qd), reference State layouts; any output NULL: skip */
+int dfx_link_state_forward(const dfx_pack_t* pack, int n, const float* q, const float* qd,
+                           float* body_X_sc, float* body_X_sm, float* body_v_s, void* stream);
+/* cotangents (NULL == 0) -> gq [n*Q], gqd [n*D] (overwritten; NULL: skip) */
+int dfx_link_state_backward(const dfx_pack_t* pack, int n, const float* q, const float* qd,
+                            const float* g_X_sc, const float* g_X_sm, const float* g_v_s,
+                            float* gq, float* gqd, void* stream);
+
 /* Launch configuration knob: lanes cooperating on one environment (8, 16 or 32; 0 = auto). */
 int dfx_set_group_size(int lanes);
 /* Tuning flags (default 9; for A/B timing and tests).  Lane-group kernels: bit 1 (2) = extra CTA-wide barriers between
