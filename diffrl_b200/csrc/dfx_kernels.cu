@@ -270,14 +270,19 @@ static int g_flags = 9;   // include/dfx.h dfx_set_flags: 2 phase barriers, 4 ge
 static int g_tape_bf16 = 0;   // dfx_set_tape_dtype
 static int g_tile_envs = 0;   // dfx_set_tile_envs: 0 = the widest tile kernel that exists for the articulation
 
+// the tile kernels of width E = 8, 16 or 32 (dfx_tile.cu)
+static const DfxTileApi* tile_api(int E) {
+    switch (E) {
+        case 8: return dfx_tile_api_e8();
+        case 16: return dfx_tile_api_e16();
+        case 32: return dfx_tile_api_e32();
+    }
+    return nullptr;
+}
+
 static int tile_mode(int E, const Pack& h) {
     if (h.jmask & ~tile_joint_mask(h.L, h.D, h.Q, h.C, h.M)) return -1;     // a joint type the tile kernels of these sizes are not compiled for
-    switch (E) {
-        case 8: return dfx_tile_mode_e8(h.L, h.D, h.Q, h.C, h.M);
-        case 16: return dfx_tile_mode_e16(h.L, h.D, h.Q, h.C, h.M);
-        case 32: return dfx_tile_mode_e32(h.L, h.D, h.Q, h.C, h.M);
-    }
-    return -1;
+    return tile_api(E)->mode(h.L, h.D, h.Q, h.C, h.M);
 }
 
 static void set_err(char* err, int n, const std::string& m) {
@@ -403,10 +408,8 @@ static int cta_area(const dfx_pack* p, int envs_per_cta) {
 // wrench: the external-wrench kernels, whose scratch ends past the layout's (dfx_pack.h wrench_scratch_end)
 static LaunchPlan plan_launch(const dfx_pack* p, int G, bool bwd, bool wrench = false) {
     LaunchPlan lp{};
-    const int per_env = wrench ? wrench_scratch_end(bwd ? p->host.layout_bwd : p->host.layout, p->header.L, bwd)
-                               : bwd ? p->host.layout_bwd.bwd_size : p->host.layout.fwd_size;
     // multiple of 4 floats (16-byte cp.async rows) that is not a multiple of 32 (bank spreading between groups)
-    lp.scratch_stride = (per_env + 3) & ~3;
+    lp.scratch_stride = scratch_floats(bwd ? p->host.layout_bwd : p->host.layout, p->header.L, bwd, wrench);
     if (lp.scratch_stride % 32 == 0) lp.scratch_stride += 4;
     lp.pack_bytes = (((p->blob.n_floats + 3) & ~3) + ((p->blob.n_ints + 3) & ~3)) * 4;
     // environments per CTA: the candidate (128, 64 or 32 threads) that keeps the most environments resident
@@ -428,30 +431,53 @@ static LaunchPlan plan_launch(const dfx_pack* p, int G, bool bwd, bool wrench = 
     return lp;
 }
 
-template <int G, bool BWD, bool WRENCH, int SL, int SD, int SQ, int SC, int SM>
-static cudaError_t launch_impl(const dfx_pack* p, const StepArgs& step, const DfxExternalWrench& w, cudaStream_t stream) {
+// the kernel argument block of a launch; the launch functions add the layout and the scratch geometry
+static KernelArgs kernel_args(const dfx_pack* p, const StepArgs& step, const DfxExternalWrench* w) {
     KernelArgs ka;
     ka.header = p->header;
     ka.blob = p->blob;
-    ka.layout = BWD ? p->host.layout_bwd : p->host.layout;
     ka.step = step;
-    ka.wrench = w;
-    const LaunchPlan lp = plan_launch(p, G, BWD, WRENCH);
+    ka.wrench = w ? *w : DfxExternalWrench{nullptr, nullptr};
+    return ka;
+}
+
+// a tile launch is counted whatever the tile function returns (also when it refuses, e.g. a wrench under flag bit 6)
+static int counted(int e) {
+    g_launches.fetch_add(1);
+    return e;
+}
+
+// the lane-group kernel families
+enum GroupFamily { kStep, kStepWrench, kLinkState };
+
+// one lane-group launch: the family's kernel of group width G, size-specialised (SL..SM > 0) or generic, with plan_launch's
+// geometry; la: the link state's kernel parameter
+template <GroupFamily F, int G, bool BWD, int SL, int SD, int SQ, int SC, int SM>
+static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const LinkStateArgs* la, cudaStream_t stream) {
+    ka.layout = BWD ? p->host.layout_bwd : p->host.layout;
+    const LaunchPlan lp = plan_launch(p, G, BWD, F == kStepWrench);
     ka.scratch_stride = lp.scratch_stride;
     ka.pack_smem_floats = lp.pack_bytes / 4;
     ka.cta_area_floats = lp.cta_area_bytes / 4;
-    const int envs_per_cta = lp.envs_per_cta;
-    if (envs_per_cta == 0) return cudaErrorInvalidConfiguration;
-    const size_t smem = lp.smem;
-    auto kern = dfx_step_kernel<G, BWD, SL, SD, SQ, SC, SM>;
-    if constexpr (WRENCH) kern = dfx_step_wrench_kernel<G, BWD, SL, SD, SQ, SC, SM>;
-    // (the opt-in to > 48 KB of dynamic shared memory is per device: set it on every launch, it is cheap)
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (step.N + envs_per_cta - 1) / envs_per_cta;
-    kern<<<grid, envs_per_cta * G, smem, stream>>>(ka);
-    g_launches.fetch_add(1);
-    return cudaGetLastError();
+    if (lp.envs_per_cta == 0) return cudaErrorInvalidConfiguration;
+    const int grid = (ka.step.N + lp.envs_per_cta - 1) / lp.envs_per_cta;
+    const auto go = [&](auto kern, const auto&... extra) {
+        // (the opt-in to > 48 KB of dynamic shared memory is per device: set it on every launch, it is cheap)
+        const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lp.smem);
+        if (e != cudaSuccess) return e;
+        kern<<<grid, lp.envs_per_cta * G, lp.smem, stream>>>(ka, extra...);
+        g_launches.fetch_add(1);
+        return cudaGetLastError();
+    };
+    if constexpr (F == kLinkState) {
+        return go(dfx_link_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *la);
+    } else {
+        // (the step kernel is referenced before its external-wrench twin, in every instantiation: nvcc emits the kernels in the
+        //  order they are first referenced, and the code of some depends on that order)
+        auto kern = dfx_step_kernel<G, BWD, SL, SD, SQ, SC, SM>;
+        if constexpr (F == kStepWrench) kern = dfx_step_wrench_kernel<G, BWD, SL, SD, SQ, SC, SM>;
+        return go(kern);
+    }
 }
 
 // the size-specialised lane-group instantiations (the six DiffRL articulations), by the group width pick_group() chooses for them
@@ -464,72 +490,18 @@ static cudaError_t launch_impl(const dfx_pack* p, const StepArgs& step, const Df
     X(22, 27, 28, 35, 0)     /* Humanoid */                                                          \
     X(11, 24, 29, 88, 152)   /* SNU humanoid (lower body, 152 muscles) */
 
-// dispatch on the model sizes: specialised instantiations for the DiffRL articulations, generic otherwise
-template <int G, bool BWD, bool WRENCH>
-static cudaError_t launch(const dfx_pack* p, const StepArgs& step, const DfxExternalWrench& w, cudaStream_t stream) {
+// dispatch on the model sizes: specialised instantiations for the DiffRL articulations, generic otherwise (and under flag bit 2)
+template <GroupFamily F, int G, bool BWD>
+static cudaError_t launch(const dfx_pack* p, KernelArgs& ka, const LinkStateArgs* la, cudaStream_t stream) {
     const Pack& h = p->header;
 #define DFX_SPECIAL(l, d, q, c, m) \
-    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return launch_impl<G, BWD, WRENCH, l, d, q, c, m>(p, step, w, stream);
+    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return launch_impl<F, G, BWD, l, d, q, c, m>(p, ka, la, stream);
     if (!(g_flags & 4)) {
         if constexpr (G == 16) { DFX_GROUP_SPECIALS_16(DFX_SPECIAL) }
         if constexpr (G == 32) { DFX_GROUP_SPECIALS_32(DFX_SPECIAL) }
     }
 #undef DFX_SPECIAL
-    return launch_impl<G, BWD, WRENCH, 0, 0, 0, 0, 0>(p, step, w, stream);
-}
-
-// the link state (dfx_link_state_kernel) with the step kernel's launch geometry for the same pass
-template <int G, bool BWD, int SL, int SD, int SQ, int SC, int SM>
-static cudaError_t link_state_launch_impl(const dfx_pack* p, int n, const LinkStateArgs& la, cudaStream_t stream) {
-    KernelArgs ka;
-    memset(&ka, 0, sizeof ka);
-    ka.header = p->header;
-    ka.blob = p->blob;
-    ka.layout = BWD ? p->host.layout_bwd : p->host.layout;
-    ka.step.N = n;
-    ka.step.flags = g_flags;
-    const LaunchPlan lp = plan_launch(p, G, BWD);
-    ka.scratch_stride = lp.scratch_stride;
-    ka.pack_smem_floats = lp.pack_bytes / 4;
-    ka.cta_area_floats = lp.cta_area_bytes / 4;
-    if (lp.envs_per_cta == 0) return cudaErrorInvalidConfiguration;
-    auto kern = dfx_link_state_kernel<G, BWD, SL, SD, SQ, SC, SM>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lp.smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (n + lp.envs_per_cta - 1) / lp.envs_per_cta;
-    kern<<<grid, lp.envs_per_cta * G, lp.smem, stream>>>(ka, la);
-    g_launches.fetch_add(1);
-    return cudaGetLastError();
-}
-
-template <int G, bool BWD>
-static cudaError_t launch_link_state(const dfx_pack* p, int n, const LinkStateArgs& la, cudaStream_t stream) {
-    const Pack& h = p->header;
-#define DFX_SPECIAL(l, d, q, c, m) \
-    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return link_state_launch_impl<G, BWD, l, d, q, c, m>(p, n, la, stream);
-    if (!(g_flags & 4)) {
-        if constexpr (G == 16) { DFX_GROUP_SPECIALS_16(DFX_SPECIAL) }
-        if constexpr (G == 32) { DFX_GROUP_SPECIALS_32(DFX_SPECIAL) }
-    }
-#undef DFX_SPECIAL
-    return link_state_launch_impl<G, BWD, 0, 0, 0, 0, 0>(p, n, la, stream);
-}
-
-static cudaError_t launch_tile(const dfx_pack* p, const StepArgs& step, bool backward, const DfxExternalWrench* w, cudaStream_t stream) {
-    KernelArgs ka;
-    ka.header = p->header;
-    ka.blob = p->blob;
-    ka.step = step;
-    ka.wrench = w ? *w : DfxExternalWrench{nullptr, nullptr};
-    const int wr = w ? 1 : 0;
-    int e = (int)cudaErrorInvalidConfiguration;
-    switch (p->tile) {
-        case 8: e = dfx_tile_launch_e8(&ka, backward, wr, stream); break;
-        case 16: e = dfx_tile_launch_e16(&ka, backward, wr, stream); break;
-        case 32: e = dfx_tile_launch_e32(&ka, backward, wr, stream); break;
-    }
-    g_launches.fetch_add(1);
-    return (cudaError_t)e;
+    return launch_impl<F, G, BWD, 0, 0, 0, 0, 0>(p, ka, la, stream);
 }
 
 static int pick_group(const dfx_pack* p) {
@@ -538,20 +510,117 @@ static int pick_group(const dfx_pack* p) {
     return widest <= 16 ? 16 : 32;
 }
 
-template <bool WRENCH>
-static int run_group(const dfx_pack_t* p, const StepArgs& a, bool backward, const DfxExternalWrench& w, cudaStream_t st) {
-    if (backward) {
-        switch (pick_group(p)) {
-            case 8: return (int)launch<8, true, WRENCH>(p, a, w, st);
-            case 16: return (int)launch<16, true, WRENCH>(p, a, w, st);
-            default: return (int)launch<32, true, WRENCH>(p, a, w, st);
-        }
-    }
+// the lane-group kernels of pick_group()'s width
+template <GroupFamily F>
+static int run_group(const dfx_pack_t* p, KernelArgs& ka, bool backward, const LinkStateArgs* la, cudaStream_t st) {
     switch (pick_group(p)) {
-        case 8: return (int)launch<8, false, WRENCH>(p, a, w, st);
-        case 16: return (int)launch<16, false, WRENCH>(p, a, w, st);
-        default: return (int)launch<32, false, WRENCH>(p, a, w, st);
+        case 8: return (int)(backward ? launch<F, 8, true>(p, ka, la, st) : launch<F, 8, false>(p, ka, la, st));
+        case 16: return (int)(backward ? launch<F, 16, true>(p, ka, la, st) : launch<F, 16, false>(p, ka, la, st));
+        default: return (int)(backward ? launch<F, 32, true>(p, ka, la, st) : launch<F, 32, false>(p, ka, la, st));
     }
+}
+
+// ---- the step entries: one set of argument checks and one StepArgs builder behind all of them
+
+// the checks every step entry starts with, and StepArgs with the env-step's sizes (false: cudaErrorInvalidValue)
+static bool step_args(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt, const DfxExternalWrench* w, StepArgs& a) {
+    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || (w && !w->f_ext)) return false;
+    memset(&a, 0, sizeof a);
+    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
+    a.dt_sub = (float)(dt / (double)substeps);
+    return true;
+}
+
+// the action map of the mapped entries, and act_other: the actuation the map does not form (muscle activations under a joint map,
+// which an articulation with muscles needs; joint actuation under a muscle map, or none)
+static bool bind_map(const dfx_pack_t* p, const DfxActionMap* m, const float* act_other, StepArgs& a) {
+    const int width = m->is_muscle ? p->header.M : p->header.D;
+    if (m->num_act <= 0 || m->offset < 0 || m->offset + m->num_act > width || !m->strength) return false;
+    if (!m->is_muscle && p->header.M > 0 && !act_other) return false;
+    a.map_num_act = m->num_act; a.map_offset = m->offset; a.map_muscle = m->is_muscle ? 1 : 0;
+    a.map_pre_scale = m->pre_scale; a.map_pre_bias = m->pre_bias; a.map_drive_scale = m->drive_scale;
+    a.strength = m->strength;
+    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
+    return true;
+}
+
+// the transition of the env-step entries: its sizes match the pack and the action map, and its rows are given
+static bool transition_sizes_ok(int kind, const DfxWalkerParams& w, const DfxPlanarParams& pl, const dfx_pack_t* p, const DfxActionMap* m) {
+    if (kind == 1) return w.num_q == p->header.Q && w.num_qd == p->header.D && w.num_act == m->num_act && w.num_obs > 0 && w.num_obs <= 96;
+    if (kind == 2) return pl.num_q == p->header.Q && pl.num_qd == p->header.D && pl.num_act == m->num_act && pl.num_obs > 0 && pl.kind >= 0 && pl.kind <= 2;
+    return false;
+}
+static bool transition_ok(const dfx_pack_t* p, const DfxActionMap* m, const DfxEnvTransition* tr) {
+    return tr && transition_sizes_ok(tr->kind, tr->walker, tr->planar, p, m) && tr->progress && tr->start_q && tr->start_qd && tr->obs_before &&
+           tr->rew && tr->reset && tr->q_next && tr->qd_next && tr->actions_next && tr->progress_next && tr->obs_next;
+}
+static bool transition_ok(const dfx_pack_t* p, const DfxActionMap* m, const DfxEnvTransitionAdj* tr) {
+    return tr && transition_sizes_ok(tr->kind, tr->walker, tr->planar, p, m) && tr->q_sim && tr->qd_sim && tr->used && tr->reset && tr->gq_sim &&
+           tr->gqd_sim && tr->g_used;
+}
+
+// the tile kernels stage the transition in dead scratch (dfx_env_dev.h tile_transition_*): is there enough of it?
+static bool transition_fits(const dfx_pack_t* p, int kind, const DfxWalkerParams& w, const DfxPlanarParams& pl, bool backward) {
+    if (!p->tile) return false;
+    const int no = kind == 1 ? w.num_obs : pl.num_obs, na = kind == 1 ? w.num_act : pl.num_act;
+    if (backward) return 2 * no + 3 * (p->header.Q + p->header.D + na) <= p->host.layout_bwd.bwd_size;
+    return 2 * no + 1 <= p->host.layout.fwd_size - p->host.layout.act;
+}
+
+// the launch-side fields of StepArgs: where the tape's H^-1 blocks start, its dtype, the flags
+static void finish_step_args(const dfx_pack_t* p, StepArgs& a) {
+    a.hinv_base = tape_geom(p->header.L, p->header.Q, p->header.D, tape_envs(p, a.N), a.substeps, a.mm_freq, p->bf16 != 0).hinv_base;
+    a.tape_bf16 = p->bf16;
+    a.flags = g_flags;
+}
+
+// w: the external wrench (NULL: none -- the kernels without one)
+static int run_step(const dfx_pack_t* p, StepArgs& a, bool backward, void* stream, const DfxExternalWrench* w = nullptr) {
+    finish_step_args(p, a);
+    KernelArgs ka = kernel_args(p, a, w);
+    if (p->tile) return counted(tile_api(p->tile)->launch(&ka, backward, w ? 1 : 0, stream));
+    cudaStream_t st = (cudaStream_t)stream;
+    return w ? run_group<kStepWrench>(p, ka, backward, nullptr, st) : run_group<kStep>(p, ka, backward, nullptr, st);
+}
+
+// end state of the recomputed forward: the workspace's tail, q [n*Q] then qd [n*D]
+static float* workspace_q_end(const dfx_pack_t* p, const StepArgs& a, float* ws) { return ws + dfx_tape_floats(p, a.N, a.substeps, a.mm_freq); }
+
+// one launch on the tile kernels: the forward into the workspace, the barrier sequence of dfx_tile_recompute_kernel, the adjoint.
+// `a` holds the adjoint's arguments (as the stored-tape entry would launch them); the forward's are added here.
+static int run_recompute_fused(const dfx_pack_t* p, StepArgs& a, const float* q, const float* qd, float* ws, void* stream,
+                               const DfxExternalWrench* w) {
+    a.q = q; a.qd = qd;
+    a.q_out = workspace_q_end(p, a, ws); a.qd_out = a.q_out + (long long)a.N * p->header.Q;
+    a.tape = ws; a.tape_in = ws;
+    a.used = nullptr; a.has_derived = 0;
+    finish_step_args(p, a);
+    KernelArgs ka = kernel_args(p, a, w);
+    return counted(tile_api(p->tile)->launch_recompute(&ka, w ? 1 : 0, stream));
+}
+
+// the fused kernel exists for every tile pack; the A/B variants of flag bit 6 have none (two launches instead)
+static bool recompute_fuses(const dfx_pack_t* p) { return p->tile != 0 && !(g_flags & 64); }
+
+// the recompute adjoint as two launches, where there is no fused kernel: forward(q_end, qd_end) writes the tape into the workspace
+// and the end state into its tail, then adjoint() runs the stored-tape entry on it
+template <class Forward, class Adjoint>
+static int recompute_in_two_launches(const dfx_pack_t* p, const StepArgs& a, float* ws, Forward forward, Adjoint adjoint) {
+    float* q_end = workspace_q_end(p, a, ws);
+    const int e = forward(q_end, q_end + (long long)a.N * p->header.Q);
+    return e != 0 ? e : adjoint();
+}
+
+// ---- link state (include/dfx.h dfx_link_state_*): the kernel family the step entries pick for the pack -- its tile kernels, or
+// the lane-group kernels of pick_group()'s width, generic under flag bit 2 (4).  The flag-64 A/B variants run the default tile
+// kernels (no tape layout to match).
+static int run_link_state(const dfx_pack_t* p, int n, const LinkStateArgs& la, bool backward, void* stream) {
+    StepArgs a{};
+    a.N = n;
+    a.flags = g_flags;
+    KernelArgs ka = kernel_args(p, a, nullptr);
+    if (p->tile) return counted(tile_api(p->tile)->launch_link_state(&ka, &la, backward, stream));
+    return run_group<kLinkState>(p, ka, backward, &la, (cudaStream_t)stream);
 }
 
 extern "C" {
@@ -560,13 +629,10 @@ int dfx_launch_plan(const dfx_pack_t* p, int backward, int out[6]) {
     if (!p || !out) return (int)cudaErrorInvalidValue;
     const bool bwd = (backward & 1) != 0, wrench = (backward & 2) != 0;
     if (p->tile) {      // one CTA = a tile of E environments
-        KernelArgs ka;
-        ka.header = p->header;
-        ka.blob = p->blob;
-        const size_t smem = p->tile == 8 ? dfx_tile_smem_e8(&ka, backward) : p->tile == 16 ? dfx_tile_smem_e16(&ka, backward) : dfx_tile_smem_e32(&ka, backward);
-        const Layout& Y = bwd ? p->host.layout_bwd : p->host.layout;
+        const KernelArgs ka = kernel_args(p, StepArgs{}, nullptr);
+        const size_t smem = tile_api(p->tile)->smem(&ka, backward);
         out[0] = 32; out[1] = p->tile; out[2] = (int)((227 * 1024) / (smem + 1024)); out[3] = (int)smem;
-        out[4] = wrench ? wrench_scratch_end(Y, p->header.L, bwd) : ((bwd ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
+        out[4] = scratch_floats(bwd ? p->host.layout_bwd : p->host.layout, p->header.L, bwd, wrench);
         out[5] = (int)smem - out[4] * p->tile * 4;
         if (wrench && smem > 227 * 1024) out[1] = 0;      // (an articulation whose external-wrench variant no longer fits)
         return 0;
@@ -578,25 +644,6 @@ int dfx_launch_plan(const dfx_pack_t* p, int backward, int out[6]) {
     return 0;
 }
 
-// w: the external wrench (NULL: none -- the kernels without one)
-static int run_step(const dfx_pack_t* p, StepArgs& a, bool backward, void* stream, const DfxExternalWrench* w = nullptr) {
-    a.hinv_base = tape_geom(p->header.L, p->header.Q, p->header.D, tape_envs(p, a.N), a.substeps, a.mm_freq, p->bf16 != 0).hinv_base;
-    a.tape_bf16 = p->bf16;
-    a.flags = g_flags;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (p->tile) return (int)launch_tile(p, a, backward, w, st);
-    return w ? run_group<true>(p, a, backward, *w, st) : run_group<false>(p, a, backward, DfxExternalWrench{nullptr, nullptr}, st);
-}
-
-static bool bind_map(const dfx_pack_t* p, const DfxActionMap* m, StepArgs& a) {
-    const int width = m->is_muscle ? p->header.M : p->header.D;
-    if (m->num_act <= 0 || m->offset < 0 || m->offset + m->num_act > width || !m->strength) return false;
-    a.map_num_act = m->num_act; a.map_offset = m->offset; a.map_muscle = m->is_muscle ? 1 : 0;
-    a.map_pre_scale = m->pre_scale; a.map_pre_bias = m->pre_bias; a.map_drive_scale = m->drive_scale;
-    a.strength = m->strength;
-    return true;
-}
-
 int dfx_step_forward(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                      const float* q, const float* qd, const float* act, const float* musc,
                      float* q_out, float* qd_out, float* tape, const DfxDerived* derived, void* stream) {
@@ -606,12 +653,9 @@ int dfx_step_forward(const dfx_pack_t* p, int n, int substeps, int mm_freq, doub
 int dfx_step_forward_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                         const float* q, const float* qd, const float* act, const float* musc,
                         float* q_out, float* qd_out, float* tape, const DfxDerived* derived, void* stream, const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
-    if (!q || !qd || !act || !q_out || !qd_out || (p->header.M > 0 && !musc)) return (int)cudaErrorInvalidValue;
     StepArgs a;
-    memset(&a, 0, sizeof a);
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !q || !qd || !act || !q_out || !qd_out || (p->header.M > 0 && !musc))
+        return (int)cudaErrorInvalidValue;
     a.q = q; a.qd = qd; a.act = act; a.musc = musc; a.q_out = q_out; a.qd_out = qd_out; a.tape = tape;
     if (derived) { a.derived = *derived; a.has_derived = 1; }
     return run_step(p, a, false, stream, w);
@@ -628,12 +672,8 @@ int dfx_step_backward_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, 
                          const float* act, const float* musc, const float* tape,
                          const float* gq_out, const float* gqd_out,
                          float* gq, float* gqd, float* gact, float* gmusc, void* stream, const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !act || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
-    if (p->header.M > 0 && !musc) return (int)cudaErrorInvalidValue;
     StepArgs a;
-    memset(&a, 0, sizeof a);
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !tape || !act || (p->header.M > 0 && !musc)) return (int)cudaErrorInvalidValue;
     a.act = act; a.musc = musc; a.tape_in = tape; a.gq_out = gq_out; a.gqd_out = gqd_out;
     a.gq = gq; a.gqd = gqd; a.gact = gact; a.gmusc = gmusc;
     return run_step(p, a, true, stream, w);
@@ -648,16 +688,10 @@ int dfx_step_forward_mapped(const dfx_pack_t* p, int n, int substeps, int mm_fre
 int dfx_step_forward_mapped_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                                const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                                float* used, float* q_out, float* qd_out, float* tape, void* stream, const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !map || !raw || !q_out || !qd_out) return (int)cudaErrorInvalidValue;
-    if (w && !w->f_ext) return (int)cudaErrorInvalidValue;
     StepArgs a;
-    memset(&a, 0, sizeof a);
-    if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
-    if (!a.map_muscle && p->header.M > 0 && !act_other) return (int)cudaErrorInvalidValue;
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !q || !qd || !map || !raw || !q_out || !qd_out || !bind_map(p, map, act_other, a))
+        return (int)cudaErrorInvalidValue;
     a.q = q; a.qd = qd; a.raw = raw; a.used = used; a.q_out = q_out; a.qd_out = qd_out; a.tape = tape;
-    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     return run_step(p, a, false, stream, w);
 }
 
@@ -673,35 +707,15 @@ int dfx_step_backward_mapped_ex(const dfx_pack_t* p, int n, int substeps, int mm
                                 const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
                                 const float* gq_out, const float* gqd_out, const float* g_used,
                                 float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !map || !raw || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
     StepArgs a;
-    memset(&a, 0, sizeof a);
-    if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
-    if (!a.map_muscle && p->header.M > 0 && !act_other) return (int)cudaErrorInvalidValue;
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !tape || !map || !raw || !bind_map(p, map, act_other, a)) return (int)cudaErrorInvalidValue;
     a.raw = raw; a.tape_in = tape; a.gq_out = gq_out; a.gqd_out = gqd_out; a.g_used = g_used;
     a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
-    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     return run_step(p, a, true, stream, w);
 }
 
 // ---- env.step() as one launch (include/dfx.h): the mapped step with the transition as epilogue (tile kernels), or the two
 // launches back to back (lane-group kernels)
-// the tile kernels stage the transition in dead scratch (dfx_env_dev.h tile_transition_*): is there enough of it?
-static bool transition_fits(const dfx_pack_t* p, int kind, const DfxWalkerParams& w, const DfxPlanarParams& pl, bool backward) {
-    if (!p->tile) return false;
-    const int no = kind == 1 ? w.num_obs : pl.num_obs, na = kind == 1 ? w.num_act : pl.num_act;
-    if (backward) return 2 * no + 3 * (p->header.Q + p->header.D + na) <= p->host.layout_bwd.bwd_size;
-    return 2 * no + 1 <= p->host.layout.fwd_size - p->host.layout.act;
-}
-
-static bool transition_ok(int kind, const DfxWalkerParams& w, const DfxPlanarParams& pl, const dfx_pack_t* p, const DfxActionMap* m) {
-    if (kind == 1) return w.num_q == p->header.Q && w.num_qd == p->header.D && w.num_act == m->num_act && w.num_obs > 0 && w.num_obs <= 96;
-    if (kind == 2) return pl.num_q == p->header.Q && pl.num_qd == p->header.D && pl.num_act == m->num_act && pl.num_obs > 0 && pl.kind >= 0 && pl.kind <= 2;
-    return false;
-}
-
 int dfx_env_step_forward(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                          const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                          float* used, float* q_sim, float* qd_sim, float* tape, const DfxEnvTransition* tr, void* stream) {
@@ -712,11 +726,9 @@ int dfx_env_step_forward_ex(const dfx_pack_t* p, int n, int substeps, int mm_fre
                             const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                             float* used, float* q_sim, float* qd_sim, float* tape, const DfxEnvTransition* tr, void* stream,
                             const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !map || !raw || !used || !q_sim || !qd_sim || !tr) return (int)cudaErrorInvalidValue;
-    if (w && !w->f_ext) return (int)cudaErrorInvalidValue;
-    if (!transition_ok(tr->kind, tr->walker, tr->planar, p, map)) return (int)cudaErrorInvalidValue;
-    if (!tr->progress || !tr->start_q || !tr->start_qd || !tr->obs_before || !tr->rew || !tr->reset || !tr->q_next || !tr->qd_next ||
-        !tr->actions_next || !tr->progress_next || !tr->obs_next) return (int)cudaErrorInvalidValue;
+    StepArgs a;
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !q || !qd || !map || !raw || !used || !q_sim || !qd_sim || !transition_ok(p, map, tr))
+        return (int)cudaErrorInvalidValue;
     if (!transition_fits(p, tr->kind, tr->walker, tr->planar, false)) {
         const int e = dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, used, q_sim, qd_sim, tape, stream, w);
         if (e != 0) return e;
@@ -726,14 +738,8 @@ int dfx_env_step_forward_ex(const dfx_pack_t* p, int n, int substeps, int mm_fre
             : dfx_planar_transition_forward(&tr->planar, n, q_sim, qd_sim, used, tr->progress, tr->start_q, tr->start_qd, tr->obs_before, tr->rew,
                                             tr->reset, tr->q_next, tr->qd_next, tr->actions_next, tr->progress_next, tr->obs_next, stream);
     }
-    StepArgs a;
-    memset(&a, 0, sizeof a);
-    if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
-    if (!a.map_muscle && p->header.M > 0 && !act_other) return (int)cudaErrorInvalidValue;
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
+    if (!bind_map(p, map, act_other, a)) return (int)cudaErrorInvalidValue;
     a.q = q; a.qd = qd; a.raw = raw; a.used = used; a.q_out = q_sim; a.qd_out = qd_sim; a.tape = tape;
-    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     a.env_kind = tr->kind;
     a.env = *tr;
     return run_step(p, a, false, stream, w);
@@ -748,9 +754,8 @@ int dfx_env_step_backward(const dfx_pack_t* p, int n, int substeps, int mm_freq,
 int dfx_env_step_backward_ex(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                              const DfxActionMap* map, const float* raw, const float* act_other, const float* tape,
                              const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !tape || !map || !raw || !tr || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
-    if (!transition_ok(tr->kind, tr->walker, tr->planar, p, map)) return (int)cudaErrorInvalidValue;
-    if (!tr->q_sim || !tr->qd_sim || !tr->used || !tr->reset || !tr->gq_sim || !tr->gqd_sim || !tr->g_used) return (int)cudaErrorInvalidValue;
+    StepArgs a;
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !tape || !map || !raw || !transition_ok(p, map, tr)) return (int)cudaErrorInvalidValue;
     if (!transition_fits(p, tr->kind, tr->walker, tr->planar, true)) {
         const int e = tr->kind == 1
             ? dfx_walker_transition_backward(&tr->walker, n, tr->q_sim, tr->qd_sim, tr->used, tr->reset, tr->g_obs_before, tr->g_rew, tr->g_q_next,
@@ -761,15 +766,9 @@ int dfx_env_step_backward_ex(const dfx_pack_t* p, int n, int substeps, int mm_fr
         return dfx_step_backward_mapped_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, tape, tr->gq_sim, tr->gqd_sim, tr->g_used, gq, gqd, g_raw,
                                            stream, w);
     }
-    StepArgs a;
-    memset(&a, 0, sizeof a);
-    if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
-    if (!a.map_muscle && p->header.M > 0 && !act_other) return (int)cudaErrorInvalidValue;
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
+    if (!bind_map(p, map, act_other, a)) return (int)cudaErrorInvalidValue;
     a.raw = raw; a.tape_in = tape; a.gq_out = tr->gq_sim; a.gqd_out = tr->gqd_sim; a.g_used = tr->g_used;
     a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
-    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     a.env_kind = tr->kind;
     a.env_adj = *tr;
     return run_step(p, a, true, stream, w);
@@ -781,39 +780,6 @@ long long dfx_recompute_workspace_floats(const dfx_pack_t* p, int n, int substep
     if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0) return -1;
     return dfx_tape_floats(p, n, substeps, mm_freq) + (long long)n * (p->header.Q + p->header.D);
 }
-
-// end state of the recomputed forward: the workspace's tail, q [n*Q] then qd [n*D]
-static float* workspace_q_end(const dfx_pack_t* p, const StepArgs& a, float* ws) { return ws + dfx_tape_floats(p, a.N, a.substeps, a.mm_freq); }
-
-// one launch on the tile kernels: the forward into the workspace, the barrier sequence of dfx_tile_recompute_kernel, the adjoint.
-// `a` holds the adjoint's arguments (as the stored-tape entry would launch them); the forward's are added here.
-static int run_recompute_fused(const dfx_pack_t* p, StepArgs& a, const float* q, const float* qd, float* ws, void* stream,
-                               const DfxExternalWrench* w) {
-    a.q = q; a.qd = qd;
-    a.q_out = workspace_q_end(p, a, ws); a.qd_out = a.q_out + (long long)a.N * p->header.Q;
-    a.tape = ws; a.tape_in = ws;
-    a.used = nullptr; a.has_derived = 0;
-    a.hinv_base = tape_geom(p->header.L, p->header.Q, p->header.D, tape_envs(p, a.N), a.substeps, a.mm_freq, p->bf16 != 0).hinv_base;
-    a.tape_bf16 = p->bf16;
-    a.flags = g_flags;
-    KernelArgs ka;
-    ka.header = p->header;
-    ka.blob = p->blob;
-    ka.step = a;
-    ka.wrench = w ? *w : DfxExternalWrench{nullptr, nullptr};
-    const int wr = w ? 1 : 0;
-    int e = (int)cudaErrorInvalidConfiguration;
-    switch (p->tile) {
-        case 8: e = dfx_tile_launch_recompute_e8(&ka, wr, stream); break;
-        case 16: e = dfx_tile_launch_recompute_e16(&ka, wr, stream); break;
-        case 32: e = dfx_tile_launch_recompute_e32(&ka, wr, stream); break;
-    }
-    g_launches.fetch_add(1);
-    return e;
-}
-
-// the fused kernel exists for every tile pack; the A/B variants of flag bit 6 have none (two launches instead)
-static bool recompute_fuses(const dfx_pack_t* p) { return p->tile != 0 && !(g_flags & 64); }
 
 int dfx_step_backward_recompute(const dfx_pack_t* p, int n, int substeps, int mm_freq, double dt,
                                 const float* q, const float* qd, const float* act, const float* musc, float* workspace,
@@ -827,19 +793,15 @@ int dfx_step_backward_recompute_ex(const dfx_pack_t* p, int n, int substeps, int
                                    const float* q, const float* qd, const float* act, const float* musc, float* workspace,
                                    const float* gq_out, const float* gqd_out,
                                    float* gq, float* gqd, float* gact, float* gmusc, void* stream, const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !act || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
-    if (p->header.M > 0 && !musc) return (int)cudaErrorInvalidValue;
     StepArgs a;
-    memset(&a, 0, sizeof a);
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
-    if (!recompute_fuses(p)) {
-        float* q_end = workspace_q_end(p, a, workspace);
-        const int e = dfx_step_forward_ex(p, n, substeps, mm_freq, dt, q, qd, act, musc, q_end, q_end + (long long)n * p->header.Q, workspace, nullptr,
-                                          stream, w);
-        if (e != 0) return e;
-        return dfx_step_backward_ex(p, n, substeps, mm_freq, dt, act, musc, workspace, gq_out, gqd_out, gq, gqd, gact, gmusc, stream, w);
-    }
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !q || !qd || !workspace || !act || (p->header.M > 0 && !musc))
+        return (int)cudaErrorInvalidValue;
+    if (!recompute_fuses(p))
+        return recompute_in_two_launches(p, a, workspace,
+            [&](float* q_end, float* qd_end) {
+                return dfx_step_forward_ex(p, n, substeps, mm_freq, dt, q, qd, act, musc, q_end, qd_end, workspace, nullptr, stream, w);
+            },
+            [&] { return dfx_step_backward_ex(p, n, substeps, mm_freq, dt, act, musc, workspace, gq_out, gqd_out, gq, gqd, gact, gmusc, stream, w); });
     a.act = act; a.musc = musc; a.gq_out = gq_out; a.gqd_out = gqd_out;
     a.gq = gq; a.gqd = gqd; a.gact = gact; a.gmusc = gmusc;
     return run_recompute_fused(p, a, q, qd, workspace, stream, w);
@@ -857,24 +819,20 @@ int dfx_step_backward_mapped_recompute_ex(const dfx_pack_t* p, int n, int subste
                                           const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                                           float* workspace, const float* gq_out, const float* gqd_out, const float* g_used,
                                           float* gq, float* gqd, float* g_raw, void* stream, const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !map || !raw || (w && !w->f_ext)) return (int)cudaErrorInvalidValue;
     StepArgs a;
-    memset(&a, 0, sizeof a);
-    if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
-    if (!a.map_muscle && p->header.M > 0 && !act_other) return (int)cudaErrorInvalidValue;
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
-    if (!recompute_fuses(p)) {
-        float* q_end = workspace_q_end(p, a, workspace);
-        const int e = dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end,
-                                                 q_end + (long long)n * p->header.Q, workspace, stream, w);
-        if (e != 0) return e;
-        return dfx_step_backward_mapped_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, gq_out, gqd_out, g_used, gq, gqd, g_raw,
-                                           stream, w);
-    }
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !q || !qd || !workspace || !map || !raw || !bind_map(p, map, act_other, a))
+        return (int)cudaErrorInvalidValue;
+    if (!recompute_fuses(p))
+        return recompute_in_two_launches(p, a, workspace, 
+            [&](float* q_end, float* qd_end) {
+                return dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end, qd_end, workspace, stream, w);
+            },
+            [&] {
+                return dfx_step_backward_mapped_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, gq_out, gqd_out, g_used, gq, gqd,
+                                                   g_raw, stream, w);
+            });
     a.raw = raw; a.gq_out = gq_out; a.gqd_out = gqd_out; a.g_used = g_used;
     a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
-    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     return run_recompute_fused(p, a, q, qd, workspace, stream, w);
 }
 
@@ -888,59 +846,23 @@ int dfx_env_step_backward_recompute_ex(const dfx_pack_t* p, int n, int substeps,
                                        const float* q, const float* qd, const DfxActionMap* map, const float* raw, const float* act_other,
                                        float* workspace, const DfxEnvTransitionAdj* tr, float* gq, float* gqd, float* g_raw, void* stream,
                                        const DfxExternalWrench* w) {
-    if (!p || n <= 0 || substeps <= 0 || mm_freq <= 0 || !q || !qd || !workspace || !map || !raw || !tr) return (int)cudaErrorInvalidValue;
-    if (w && !w->f_ext) return (int)cudaErrorInvalidValue;
-    if (!transition_ok(tr->kind, tr->walker, tr->planar, p, map)) return (int)cudaErrorInvalidValue;
-    if (!tr->q_sim || !tr->qd_sim || !tr->used || !tr->reset || !tr->gq_sim || !tr->gqd_sim || !tr->g_used) return (int)cudaErrorInvalidValue;
     StepArgs a;
-    memset(&a, 0, sizeof a);
-    if (!bind_map(p, map, a)) return (int)cudaErrorInvalidValue;
-    if (!a.map_muscle && p->header.M > 0 && !act_other) return (int)cudaErrorInvalidValue;
-    a.N = n; a.substeps = substeps; a.mm_freq = mm_freq;
-    a.dt_sub = (float)(dt / (double)substeps);
-    if (!recompute_fuses(p) || !transition_fits(p, tr->kind, tr->walker, tr->planar, true)) {
-        // the plain mapped forward (the transition's outputs are not needed again: its adjoint reads tr->q_sim, ...), then the
-        // stored-tape entry, which runs the transition adjoint as its prologue or as a launch of its own
-        float* q_end = workspace_q_end(p, a, workspace);
-        const int e = dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end,
-                                                 q_end + (long long)n * p->header.Q, workspace, stream, w);
-        if (e != 0) return e;
-        return dfx_env_step_backward_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, tr, gq, gqd, g_raw, stream, w);
-    }
+    if (!step_args(p, n, substeps, mm_freq, dt, w, a) || !q || !qd || !workspace || !map || !raw || !transition_ok(p, map, tr) ||
+        !bind_map(p, map, act_other, a))
+        return (int)cudaErrorInvalidValue;
+    // (the stored-tape entry runs the transition adjoint as its prologue or as a launch of its own; the forward needs none of the
+    //  transition's outputs: its adjoint reads tr->q_sim, ...)
+    if (!recompute_fuses(p) || !transition_fits(p, tr->kind, tr->walker, tr->planar, true))
+        return recompute_in_two_launches(p, a, workspace, 
+            [&](float* q_end, float* qd_end) {
+                return dfx_step_forward_mapped_ex(p, n, substeps, mm_freq, dt, q, qd, map, raw, act_other, nullptr, q_end, qd_end, workspace, stream, w);
+            },
+            [&] { return dfx_env_step_backward_ex(p, n, substeps, mm_freq, dt, map, raw, act_other, workspace, tr, gq, gqd, g_raw, stream, w); });
     a.raw = raw; a.gq_out = tr->gq_sim; a.gqd_out = tr->gqd_sim; a.g_used = tr->g_used;
     a.gq = gq; a.gqd = gqd; a.g_raw = g_raw;
-    if (a.map_muscle) a.act = act_other; else a.musc = act_other;
     a.env_kind = tr->kind;
     a.env_adj = *tr;
     return run_recompute_fused(p, a, q, qd, workspace, stream, w);
-}
-
-// ---- link state (include/dfx.h dfx_link_state_*): the kernel family the step entries pick for the pack -- its tile kernels, or
-// the lane-group kernels of pick_group()'s width, generic under flag bit 2 (4).  The flag-64 A/B variants run the default tile
-// kernels (no tape layout to match).
-static int run_link_state(const dfx_pack_t* p, int n, const LinkStateArgs& la, bool backward, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (p->tile) {
-        KernelArgs ka;
-        memset(&ka, 0, sizeof ka);
-        ka.header = p->header;
-        ka.blob = p->blob;
-        ka.step.N = n;
-        ka.step.flags = g_flags;
-        int e = (int)cudaErrorInvalidConfiguration;
-        switch (p->tile) {
-            case 8: e = dfx_tile_launch_link_state_e8(&ka, &la, backward, stream); break;
-            case 16: e = dfx_tile_launch_link_state_e16(&ka, &la, backward, stream); break;
-            case 32: e = dfx_tile_launch_link_state_e32(&ka, &la, backward, stream); break;
-        }
-        g_launches.fetch_add(1);
-        return e;
-    }
-    switch (pick_group(p)) {
-        case 8: return (int)(backward ? launch_link_state<8, true>(p, n, la, st) : launch_link_state<8, false>(p, n, la, st));
-        case 16: return (int)(backward ? launch_link_state<16, true>(p, n, la, st) : launch_link_state<16, false>(p, n, la, st));
-        default: return (int)(backward ? launch_link_state<32, true>(p, n, la, st) : launch_link_state<32, false>(p, n, la, st));
-    }
 }
 
 int dfx_link_state_forward(const dfx_pack_t* p, int n, const float* q, const float* qd,

@@ -66,21 +66,23 @@ struct KernelArgs {
     DfxExternalWrench wrench;   // read by the external-wrench kernels only (last: the other fields keep their offsets)
 };
 
+// floats of scratch per environment of a step kernel in layout Y: the layout's forward or backward size, rounded to whole 16-byte
+// rows; the external-wrench kernels' scratch ends past it (dfx_pack.h wrench_scratch_end)
+DFX_LAYOUT_FN int scratch_floats(const Layout& Y, int L, bool bwd, bool wrench) {
+    return wrench ? wrench_scratch_end(Y, L, bwd) : ((bwd ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
+}
 
 }  // namespace dfx
 
 // ---- tile kernels (dfx_tile.cu, compiled once per tile width E = 8, 16, 32 with its own namespace): one CTA = E
 // environments.  KernelArgs is a plain struct with the same layout in every build; it crosses as void*.
-#define DFX_DECLARE_TILE(E)                                                                                           \
-    int dfx_tile_mode_e##E(int L, int D, int Q, int C, int M);      /* layout mode, or -1: no kernel of this width */  \
-    /* dynamic shared memory (bytes); backward: bit 0 adjoint, bit 1 the external-wrench variant */                   \
-    size_t dfx_tile_smem_e##E(const void* kernel_args, int backward);                                                \
-    /* wrench != 0: the external-wrench kernels (kernel_args' `wrench`) */                                             \
-    int dfx_tile_launch_e##E(void* kernel_args, int backward, int wrench, void* stream);                             \
-    int dfx_tile_launch_recompute_e##E(void* kernel_args, int wrench, void* stream);   /* forward into the workspace + adjoint, one launch */ \
-    /* the link state (link_args: a LinkStateArgs); backward != 0: its adjoint */                                     \
-    int dfx_tile_launch_link_state_e##E(void* kernel_args, const void* link_args, int backward, void* stream);
-DFX_DECLARE_TILE(8)
-DFX_DECLARE_TILE(16)
-DFX_DECLARE_TILE(32)
-#undef DFX_DECLARE_TILE
+struct DfxTileApi {
+    int (*mode)(int L, int D, int Q, int C, int M);      // layout mode, or -1: no kernel of this width
+    size_t (*smem)(const void* kernel_args, int backward);   // dynamic shared memory (bytes); backward: bit 0 adjoint, bit 1 wrench
+    int (*launch)(void* kernel_args, int backward, int wrench, void* stream);   // wrench != 0: the external-wrench kernels
+    int (*launch_recompute)(void* kernel_args, int wrench, void* stream);       // forward into the workspace + adjoint, one launch
+    int (*launch_link_state)(void* kernel_args, const void* link_args, int backward, void* stream);   // link_args: a LinkStateArgs
+};
+const DfxTileApi* dfx_tile_api_e8(void);
+const DfxTileApi* dfx_tile_api_e16(void);
+const DfxTileApi* dfx_tile_api_e32(void);

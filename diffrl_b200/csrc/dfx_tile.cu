@@ -451,62 +451,64 @@ static int tile_pack_floats(const KernelArgs& ka) {
 }
 // CTA area: 4 ints (task counter, cursor), 2 mbarriers (16 bytes), then one list slot per (contact point, environment)
 static int tile_area_floats(const KernelArgs& ka) { return ((32 + ka.header.C * DFX_TILE_E * 4 + 127) & ~127) / 4; }
+// dynamic shared memory of a tile kernel (bytes): pack + CTA area + E x scratch (per_env floats per environment)
+static size_t tile_smem_bytes(const KernelArgs& ka, int per_env) {
+    return (size_t)(tile_pack_floats(ka) + tile_area_floats(ka) + per_env * DFX_TILE_E) * sizeof(float);
+}
 
-template <int NW, int MINB, bool BWD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM, bool WRENCH>
-static cudaError_t tile_launch_impl(KernelArgs& ka, cudaStream_t stream) {
-    constexpr Layout Y = make_layout(SL, SD, SQ, SC, SM, MODE, BWD);
-    const int per_env = WRENCH ? wrench_scratch_end(Y, SL, BWD) : ((BWD ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
+// one tile launch: kernel `kern` of NW warps, with layout Y and per_env scratch floats per environment, over ceil(N / E) CTAs;
+// `extra` is the kernel's parameter after KernelArgs, if it has one
+template <int NW, class... P, class... A>
+static cudaError_t tile_launch(void (*kern)(P...), const Layout& Y, int per_env, KernelArgs& ka, cudaStream_t stream, const A&... extra) {
     ka.layout = Y;
     ka.pack_smem_floats = tile_pack_floats(ka);
     ka.cta_area_floats = tile_area_floats(ka);
     ka.scratch_stride = per_env;
-    const size_t smem = (size_t)(ka.pack_smem_floats + ka.cta_area_floats + per_env * DFX_TILE_E) * sizeof(float);
-    auto kern = dfx_tile_kernel<NW, MINB, BWD, PATH, MODE, SL, SD, SQ, SC, SM>;
-    if constexpr (WRENCH) kern = dfx_tile_wrench_kernel<NW, MINB, BWD, PATH, MODE, SL, SD, SQ, SC, SM>;
+    const size_t smem = tile_smem_bytes(ka, per_env);
     // (the opt-in to > 48 KB of dynamic shared memory is per device: set it on every launch, it is cheap)
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     const int ntiles = (ka.step.N + DFX_TILE_E - 1) / DFX_TILE_E;
-    kern<<<ntiles, NW * 32, smem, stream>>>(ka);
+    kern<<<ntiles, NW * 32, smem, stream>>>(ka, extra...);
     return cudaGetLastError();
 }
 
-template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM, bool WRENCH>
-static cudaError_t tile_recompute_launch_impl(KernelArgs& ka, cudaStream_t stream) {
-    constexpr Layout YF = make_layout(SL, SD, SQ, SC, SM, MODE, false);
-    constexpr Layout YB = make_layout(SL, SD, SQ, SC, SM, MODE, true);
-    const int per_env = WRENCH ? dfx_max(wrench_scratch_end(YF, SL, false), wrench_scratch_end(YB, SL, true))
-                               : ((YF.fwd_size > YB.bwd_size ? YF.fwd_size : YB.bwd_size) + 3) & ~3;
-    ka.layout = YB;
-    ka.pack_smem_floats = tile_pack_floats(ka);
-    ka.cta_area_floats = tile_area_floats(ka);
-    ka.scratch_stride = per_env;
-    const size_t smem = (size_t)(ka.pack_smem_floats + ka.cta_area_floats + per_env * DFX_TILE_E) * sizeof(float);
-    auto kern = dfx_tile_recompute_kernel<NW, MINB, PATH, MODE, SL, SD, SQ, SC, SM>;
-    if constexpr (WRENCH) kern = dfx_tile_recompute_wrench_kernel<NW, MINB, PATH, MODE, SL, SD, SQ, SC, SM>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int ntiles = (ka.step.N + DFX_TILE_E - 1) / DFX_TILE_E;
-    kern<<<ntiles, NW * 32, smem, stream>>>(ka);
-    return cudaGetLastError();
-}
+// what a tile entry point asks of the articulation's model entry (below): its layout mode, or a launch of one of its kernels
+enum class TileOp { mode, step, recompute, link_state };
+struct TileCall {
+    TileOp op;
+    bool backward, wrench;
+    KernelArgs* ka;
+    const LinkStateArgs* la;
+    cudaStream_t stream;
+};
 
-// the step kernel's scratch (same layout, no tape): whatever the step fits, this fits
-template <int NW, int MINB, bool BWD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
-static cudaError_t tile_link_state_launch_impl(KernelArgs& ka, const LinkStateArgs& la, cudaStream_t stream) {
-    constexpr Layout Y = make_layout(SL, SD, SQ, SC, SM, MODE, BWD);
-    const int per_env = ((BWD ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
-    ka.layout = Y;
-    ka.pack_smem_floats = tile_pack_floats(ka);
-    ka.cta_area_floats = tile_area_floats(ka);
-    ka.scratch_stride = per_env;
-    const size_t smem = (size_t)(ka.pack_smem_floats + ka.cta_area_floats + per_env * DFX_TILE_E) * sizeof(float);
-    auto kern = dfx_tile_link_state_kernel<NW, MINB, BWD, PATH, MODE, SL, SD, SQ, SC, SM>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int ntiles = (ka.step.N + DFX_TILE_E - 1) / DFX_TILE_E;
-    kern<<<ntiles, NW * 32, smem, stream>>>(ka, la);
-    return cudaGetLastError();
+// one model entry (X(...) of DFX_TILE_MODELS below); ALT: an entry of DFX_TILE_MODELS_ALT, which has the step kernels only.
+// The recompute adjoint runs with the backward kernel's warps and occupancy (every entry has as many forward as backward warps;
+// tuning builds that set them apart run the forward part with the backward's) and scratch for the larger of the two layouts.
+template <int NWF, int NWB, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM, bool ALT>
+static int tile_model(const TileCall& c) {
+    if (c.op == TileOp::mode) return MODE;
+    constexpr int LM = MODE & 3;
+    constexpr Layout YF = make_layout(SL, SD, SQ, SC, SM, LM, false), YB = make_layout(SL, SD, SQ, SC, SM, LM, true);
+    const int per_f = scratch_floats(YF, SL, false, c.wrench), per_b = scratch_floats(YB, SL, true, c.wrench);
+    KernelArgs& ka = *c.ka;
+    // (kernels referenced in the order of the step, its external-wrench twin, the recompute adjoint, the link state: nvcc emits
+    //  the kernels in the order they are first referenced, and the code of some depends on that order)
+    if (c.op == TileOp::step && !c.wrench)
+        return c.backward ? tile_launch<NWB>(dfx_tile_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream)
+                          : tile_launch<NWF>(dfx_tile_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream);
+    if constexpr (!ALT) {
+        if (c.op == TileOp::step)
+            return c.backward ? tile_launch<NWB>(dfx_tile_wrench_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream)
+                              : tile_launch<NWF>(dfx_tile_wrench_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream);
+        if (c.op == TileOp::recompute)
+            return c.wrench ? tile_launch<NWB>(dfx_tile_recompute_wrench_kernel<NWB, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YB, dfx_max(per_f, per_b), ka, c.stream)
+                            : tile_launch<NWB>(dfx_tile_recompute_kernel<NWB, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YB, dfx_max(per_f, per_b), ka, c.stream);
+        return c.backward ? tile_launch<NWB>(dfx_tile_link_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, *c.la)
+                          : tile_launch<NWF>(dfx_tile_link_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, *c.la);
+    }
+    return -1;      // (the A/B variants are asked for the step only)
 }
 
 }  // namespace dfx
@@ -556,77 +558,60 @@ using namespace dfx;
 #define DFX_CAT(a, b) DFX_CAT2(a, b)
 #define DFX_TILE_FN(name) DFX_CAT(DFX_CAT(name, _e), DFX_TILE_E)
 
-// layout mode of the tile kernel for this articulation (bit 4 (16): instantiated for A/B runs only, never picked
-// automatically), or -1 when there is none of this width
-int DFX_TILE_FN(dfx_tile_mode)(int L, int D, int Q, int C, int M) {
-#define X(nwf, nwb, minb, path, mode, l, d, q, c, m) if (L == l && D == d && Q == q && C == c && M == m) return mode;
-    DFX_TILE_MODELS(X)
+// tile_model() of the articulation's entry in DFX_TILE_MODELS (ALT: DFX_TILE_MODELS_ALT), or -1 when it has none
+template <bool ALT>
+static int tile_dispatch(int L, int D, int Q, int C, int M, const TileCall& call) {
+#define X(nwf, nwb, minb, path, mode, l, d, q, c, m) \
+    if (L == l && D == d && Q == q && C == c && M == m) return tile_model<nwf, nwb, minb, path, mode, l, d, q, c, m, ALT>(call);
+    if constexpr (ALT) { DFX_TILE_MODELS_ALT(X) } else { DFX_TILE_MODELS(X) }
 #undef X
     return -1;
 }
 
-// dynamic shared memory of the tile kernel (bytes): pack + CTA area + E x scratch
-size_t DFX_TILE_FN(dfx_tile_smem)(const void* kargs, int backward) {
+// a launch on the articulation's kernels; alt: the A/B variant of flag bit 6 (64) where it has one, the default kernels otherwise
+static int tile_run(const TileCall& call, bool alt) {
+    const Pack& h = call.ka->header;
+    int e = alt ? tile_dispatch<true>(h.L, h.D, h.Q, h.C, h.M, call) : -1;
+    if (e < 0) e = tile_dispatch<false>(h.L, h.D, h.Q, h.C, h.M, call);
+    return e < 0 ? (int)cudaErrorInvalidConfiguration : e;
+}
+
+// layout mode of the tile kernel for this articulation (bit 4 (16): instantiated for A/B runs only, never picked
+// automatically), or -1 when there is none of this width
+static int tile_mode(int L, int D, int Q, int C, int M) { return tile_dispatch<false>(L, D, Q, C, M, TileCall{TileOp::mode}); }
+
+// dynamic shared memory of the tile kernel (bytes); backward: bit 0 adjoint, bit 1 the external-wrench variant
+static size_t tile_smem(const void* kargs, int backward) {
     const KernelArgs& ka = *static_cast<const KernelArgs*>(kargs);
-    const int mode = DFX_TILE_FN(dfx_tile_mode)(ka.header.L, ka.header.D, ka.header.Q, ka.header.C, ka.header.M);
+    const Pack& h = ka.header;
+    const int mode = tile_mode(h.L, h.D, h.Q, h.C, h.M);
     const bool bwd = (backward & 1) != 0;
-    const Layout Y = make_layout(ka.header.L, ka.header.D, ka.header.Q, ka.header.C, ka.header.M, mode < 0 ? 0 : (mode & 3), bwd);
-    const int per_env = (backward & 2) ? wrench_scratch_end(Y, ka.header.L, bwd) : ((bwd ? Y.bwd_size : Y.fwd_size) + 3) & ~3;
-    return (size_t)(tile_pack_floats(ka) + tile_area_floats(ka) + per_env * DFX_TILE_E) * sizeof(float);
+    const Layout Y = make_layout(h.L, h.D, h.Q, h.C, h.M, mode < 0 ? 0 : (mode & 3), bwd);
+    return tile_smem_bytes(ka, scratch_floats(Y, h.L, bwd, (backward & 2) != 0));
 }
 
-int DFX_TILE_FN(dfx_tile_launch)(void* kargs, int backward, int wrench, void* stream) {
-    KernelArgs& ka = *static_cast<KernelArgs*>(kargs);
-    const Pack& h = ka.header;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
-    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
-        return (int)(backward ? tile_launch_impl<nwb, minb, true, path, (mode) & 3, l, d, q, c, m, false>(ka, st)   \
-                              : tile_launch_impl<nwf, minb, false, path, (mode) & 3, l, d, q, c, m, false>(ka, st));
-    // (the flag-64 A/B variants have no external-wrench kernels: cudaErrorNotSupported below)
-    if (ka.step.flags & 64) {
-        if (wrench) return (int)cudaErrorNotSupported;
-        DFX_TILE_MODELS_ALT(X)
-    }
-    if (!wrench) { DFX_TILE_MODELS(X) }
-#undef X
-#define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
-    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
-        return (int)(backward ? tile_launch_impl<nwb, minb, true, path, (mode) & 3, l, d, q, c, m, true>(ka, st)   \
-                              : tile_launch_impl<nwf, minb, false, path, (mode) & 3, l, d, q, c, m, true>(ka, st));
-    if (wrench) { DFX_TILE_MODELS(X) }
-#undef X
-    return (int)cudaErrorInvalidConfiguration;
+// the step or its adjoint; wrench != 0: the external-wrench kernels (the flag-64 A/B variants have none)
+static int tile_launch_step(void* kargs, int backward, int wrench, void* stream) {
+    KernelArgs* ka = static_cast<KernelArgs*>(kargs);
+    const bool alt = (ka->step.flags & 64) != 0;
+    if (alt && wrench) return (int)cudaErrorNotSupported;
+    return tile_run(TileCall{TileOp::step, backward != 0, wrench != 0, ka, nullptr, static_cast<cudaStream_t>(stream)}, alt);
 }
 
-// the recompute adjoint (dfx_tile_recompute_kernel) of every DFX_TILE_MODELS entry, with the backward kernel's warps and
-// occupancy (every entry has as many forward as backward warps; tuning builds that set them apart run the forward part with
-// the backward's).  No flag-64 (A/B) variants: the caller runs the forward and the backward launches instead.
-int DFX_TILE_FN(dfx_tile_launch_recompute)(void* kargs, int wrench, void* stream) {
-    KernelArgs& ka = *static_cast<KernelArgs*>(kargs);
-    const Pack& h = ka.header;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
-    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
-        return (int)(wrench ? tile_recompute_launch_impl<nwb, minb, path, (mode) & 3, l, d, q, c, m, true>(ka, st)   \
-                            : tile_recompute_launch_impl<nwb, minb, path, (mode) & 3, l, d, q, c, m, false>(ka, st));
-    DFX_TILE_MODELS(X)
-#undef X
-    return (int)cudaErrorInvalidConfiguration;
+// the recompute adjoint (dfx_tile_recompute_kernel).  No flag-64 (A/B) variants: the caller runs the forward and the backward
+// launches instead.
+static int tile_launch_recompute(void* kargs, int wrench, void* stream) {
+    return tile_run(TileCall{TileOp::recompute, true, wrench != 0, static_cast<KernelArgs*>(kargs), nullptr, static_cast<cudaStream_t>(stream)}, false);
 }
 
-// the link state (dfx_tile_link_state_kernel) of every DFX_TILE_MODELS entry, with the step kernels' warps and occupancy.  The
-// flag-64 (A/B) variants have none: they run these, which is valid because the link state has no tape layout to match.
-int DFX_TILE_FN(dfx_tile_launch_link_state)(void* kargs, const void* largs, int backward, void* stream) {
-    KernelArgs& ka = *static_cast<KernelArgs*>(kargs);
-    const LinkStateArgs& la = *static_cast<const LinkStateArgs*>(largs);
-    const Pack& h = ka.header;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define X(nwf, nwb, minb, path, mode, l, d, q, c, m)                                                   \
-    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m)                                      \
-        return (int)(backward ? tile_link_state_launch_impl<nwb, minb, true, path, (mode) & 3, l, d, q, c, m>(ka, la, st)   \
-                              : tile_link_state_launch_impl<nwf, minb, false, path, (mode) & 3, l, d, q, c, m>(ka, la, st));
-    DFX_TILE_MODELS(X)
-#undef X
-    return (int)cudaErrorInvalidConfiguration;
+// the link state (dfx_tile_link_state_kernel) with the step kernels' warps and occupancy.  The flag-64 (A/B) variants have none:
+// they run these, which is valid because the link state has no tape layout to match.
+static int tile_launch_link_state(void* kargs, const void* largs, int backward, void* stream) {
+    return tile_run(TileCall{TileOp::link_state, backward != 0, false, static_cast<KernelArgs*>(kargs), static_cast<const LinkStateArgs*>(largs),
+                             static_cast<cudaStream_t>(stream)}, false);
+}
+
+const DfxTileApi* DFX_TILE_FN(dfx_tile_api)(void) {
+    static const DfxTileApi api = {tile_mode, tile_smem, tile_launch_step, tile_launch_recompute, tile_launch_link_state};
+    return &api;
 }
