@@ -52,3 +52,26 @@ def link_state(model, joint_q, joint_qd):
 
 
 LinkState = collections.namedtuple("LinkState", ["body_X_sc", "body_X_sm", "body_v_s"])
+
+
+def contact_state(model, joint_q, joint_qd):
+    """What the ground does to the links at the state (joint_q, joint_qd) of ``model``'s N environments, differentiable:
+    ``ContactState(contact_f, contact_height, body_f_contact)``, fp32, world axes --
+
+    - ``contact_f`` [N, C, 3]: the force the ground exerts on the link at each contact point, in the Model's contact order
+      (``contact_body0``); zero for a point that does not penetrate, and for every point when ``model.ground`` is off;
+    - ``contact_height`` [N, C]: the point's signed height above the plane, (X_sc p0).y - contact_dist, negative when
+      penetrating (computed with the ground on or off);
+    - ``body_f_contact`` [N, L, 6]: per link, (torque about its centre of mass, force) summed over its points -- the ``f_ext``
+      convention, so it can be passed back as an external wrench.
+
+    This is the step's own penalty contact model at the given state: what the first substep of an env-step from it applies.
+    One kernel launch forward (include/dfx.h dfx_contact_state_forward) and one backward, which recomputes the kinematics from
+    (joint_q, joint_qd).  The force's gradient flows through penetrating points only, the height's through every point.
+    joint_q [N*Q] or [N, Q], joint_qd [N*D] or [N, D], fp32 on the model's device (ValueError otherwise)."""
+    from .dflex_api.sim import _engine_for
+    from .engine import ContactStateFunction
+    return ContactState(*ContactStateFunction.apply(_engine_for(model), joint_q, joint_qd))
+
+
+ContactState = collections.namedtuple("ContactState", ["contact_f", "contact_height", "body_f_contact"])

@@ -245,6 +245,45 @@ __global__ void __launch_bounds__(kMaxThreads) dfx_link_state_kernel(const __gri
     else link_state_forward(P, Y, s, g, env, la);
 }
 
+// Contact state (include/dfx.h dfx_contact_state_forward / _backward; dfx_step.h contact_state_*): the set-up of
+// dfx_link_state_kernel line for line (keep the two in step), then the ground-contact model at (q, qd) or its adjoint.  (One kernel
+// templated on the readout would rename the link-state kernels and change their code: the set-up is written out per kernel.)
+template <int G, bool BACKWARD, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(kMaxThreads) dfx_contact_state_kernel(const __grid_constant__ KernelArgs ka,
+                                                                      const __grid_constant__ ContactStateArgs ca) {
+    extern __shared__ __align__(16) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += blockDim.x) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += blockDim.x) ipack[i] = ka.blob.ints[i];
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    Layout Y = ka.layout;
+    if constexpr (SL > 0) {
+        P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+        constexpr Layout kY = make_layout(SL, SD, SQ, SC, SM);
+        Y = kY;
+    }
+    const int kEnvsPerCta = blockDim.x / G;
+    const int local = threadIdx.x / G;
+    int env = blockIdx.x * kEnvsPerCta + local;      // (groups past the end redo the last environment, as in step_kernel_body)
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const int lane_in_warp = threadIdx.x & 31;
+    GroupCuda<G> g;
+    g.lane = threadIdx.x % G;
+    g.psync = (ka.step.flags & 2) != 0;
+    g.mask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << ((lane_in_warp / G) * G));
+    float* s = smem + ka.pack_smem_floats + ka.cta_area_floats + (size_t)local * ka.scratch_stride;
+    g.scratch0 = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    g.task_count = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    g.task_list = g.task_count + 4;
+    g.stride = ka.scratch_stride;
+    g.envs_shift = 31 - __clz(kEnvsPerCta > 0 ? kEnvsPerCta : 1);
+    g.cta_mode = (ka.step.flags & 8) != 0;
+    if (BACKWARD) contact_state_backward(P, Y, s, g, env, ca);
+    else contact_state_forward(P, Y, s, g, env, ca);
+}
+
 }  // namespace dfx
 
 // =====================================================================================
@@ -259,6 +298,7 @@ struct dfx_pack {
     int device;
     int* d_ints;
     float* d_floats;
+    int* d_corder;   // [C]: Model index of the pack's contact n (the contact state's outputs are in the Model's order)
     Pack header;
     PackBlob blob;
 };
@@ -332,6 +372,9 @@ dfx_pack_t* dfx_pack_create(const DfxModelDesc* desc, int device, char* err, int
     if (e == cudaSuccess) e = cudaMalloc(&p->d_floats, p->host.floats.size() * sizeof(float) + 16);
     if (e == cudaSuccess) e = cudaMemcpy(p->d_ints, p->host.ints.data(), p->host.ints.size() * sizeof(int), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(p->d_floats, p->host.floats.data(), p->host.floats.size() * sizeof(float), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMalloc(&p->d_corder, p->host.corder.size() * sizeof(int) + 16);
+    if (e == cudaSuccess && !p->host.corder.empty())
+        e = cudaMemcpy(p->d_corder, p->host.corder.data(), p->host.corder.size() * sizeof(int), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) { set_err(err, err_len, std::string("CUDA: ") + cudaGetErrorString(e)); delete p; return nullptr; }
     p->header = p->host.header;
     p->blob.ints = p->d_ints; p->blob.floats = p->d_floats;
@@ -359,6 +402,7 @@ void dfx_pack_destroy(dfx_pack_t* p) {
     if (!p) return;
     cudaFree(p->d_ints);
     cudaFree(p->d_floats);
+    cudaFree(p->d_corder);
     delete p;
 }
 
@@ -448,12 +492,12 @@ static int counted(int e) {
 }
 
 // the lane-group kernel families
-enum GroupFamily { kStep, kStepWrench, kLinkState };
+enum GroupFamily { kStep, kStepWrench, kLinkState, kContactState };
 
 // one lane-group launch: the family's kernel of group width G, size-specialised (SL..SM > 0) or generic, with plan_launch's
-// geometry; la: the link state's kernel parameter
+// geometry; ra: the readout's kernel parameter (a LinkStateArgs or a ContactStateArgs), NULL for the step families
 template <GroupFamily F, int G, bool BWD, int SL, int SD, int SQ, int SC, int SM>
-static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const LinkStateArgs* la, cudaStream_t stream) {
+static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const void* ra, cudaStream_t stream) {
     ka.layout = BWD ? p->host.layout_bwd : p->host.layout;
     const LaunchPlan lp = plan_launch(p, G, BWD, F == kStepWrench);
     ka.scratch_stride = lp.scratch_stride;
@@ -470,7 +514,9 @@ static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const LinkStat
         return cudaGetLastError();
     };
     if constexpr (F == kLinkState) {
-        return go(dfx_link_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *la);
+        return go(dfx_link_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *static_cast<const LinkStateArgs*>(ra));
+    } else if constexpr (F == kContactState) {
+        return go(dfx_contact_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *static_cast<const ContactStateArgs*>(ra));
     } else {
         // (the step kernel is referenced before its external-wrench twin, in every instantiation: nvcc emits the kernels in the
         //  order they are first referenced, and the code of some depends on that order)
@@ -492,16 +538,16 @@ static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const LinkStat
 
 // dispatch on the model sizes: specialised instantiations for the DiffRL articulations, generic otherwise (and under flag bit 2)
 template <GroupFamily F, int G, bool BWD>
-static cudaError_t launch(const dfx_pack* p, KernelArgs& ka, const LinkStateArgs* la, cudaStream_t stream) {
+static cudaError_t launch(const dfx_pack* p, KernelArgs& ka, const void* ra, cudaStream_t stream) {
     const Pack& h = p->header;
 #define DFX_SPECIAL(l, d, q, c, m) \
-    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return launch_impl<F, G, BWD, l, d, q, c, m>(p, ka, la, stream);
+    if (h.L == l && h.D == d && h.Q == q && h.C == c && h.M == m) return launch_impl<F, G, BWD, l, d, q, c, m>(p, ka, ra, stream);
     if (!(g_flags & 4)) {
         if constexpr (G == 16) { DFX_GROUP_SPECIALS_16(DFX_SPECIAL) }
         if constexpr (G == 32) { DFX_GROUP_SPECIALS_32(DFX_SPECIAL) }
     }
 #undef DFX_SPECIAL
-    return launch_impl<F, G, BWD, 0, 0, 0, 0, 0>(p, ka, la, stream);
+    return launch_impl<F, G, BWD, 0, 0, 0, 0, 0>(p, ka, ra, stream);
 }
 
 static int pick_group(const dfx_pack* p) {
@@ -512,11 +558,11 @@ static int pick_group(const dfx_pack* p) {
 
 // the lane-group kernels of pick_group()'s width
 template <GroupFamily F>
-static int run_group(const dfx_pack_t* p, KernelArgs& ka, bool backward, const LinkStateArgs* la, cudaStream_t st) {
+static int run_group(const dfx_pack_t* p, KernelArgs& ka, bool backward, const void* ra, cudaStream_t st) {
     switch (pick_group(p)) {
-        case 8: return (int)(backward ? launch<F, 8, true>(p, ka, la, st) : launch<F, 8, false>(p, ka, la, st));
-        case 16: return (int)(backward ? launch<F, 16, true>(p, ka, la, st) : launch<F, 16, false>(p, ka, la, st));
-        default: return (int)(backward ? launch<F, 32, true>(p, ka, la, st) : launch<F, 32, false>(p, ka, la, st));
+        case 8: return (int)(backward ? launch<F, 8, true>(p, ka, ra, st) : launch<F, 8, false>(p, ka, ra, st));
+        case 16: return (int)(backward ? launch<F, 16, true>(p, ka, ra, st) : launch<F, 16, false>(p, ka, ra, st));
+        default: return (int)(backward ? launch<F, 32, true>(p, ka, ra, st) : launch<F, 32, false>(p, ka, ra, st));
     }
 }
 
@@ -619,8 +665,18 @@ static int run_link_state(const dfx_pack_t* p, int n, const LinkStateArgs& la, b
     a.N = n;
     a.flags = g_flags;
     KernelArgs ka = kernel_args(p, a, nullptr);
-    if (p->tile) return counted(tile_api(p->tile)->launch_link_state(&ka, &la, backward, stream));
+    if (p->tile) return counted(tile_api(p->tile)->launch_readout(&ka, kReadoutLinkState, &la, backward, stream));
     return run_group<kLinkState>(p, ka, backward, &la, (cudaStream_t)stream);
+}
+
+// ---- contact state (include/dfx.h dfx_contact_state_*): on the kernels run_link_state picks
+static int run_contact_state(const dfx_pack_t* p, int n, const ContactStateArgs& ca, bool backward, void* stream) {
+    StepArgs a{};
+    a.N = n;
+    a.flags = g_flags;
+    KernelArgs ka = kernel_args(p, a, nullptr);
+    if (p->tile) return counted(tile_api(p->tile)->launch_readout(&ka, kReadoutContactState, &ca, backward, stream));
+    return run_group<kContactState>(p, ka, backward, &ca, (cudaStream_t)stream);
 }
 
 extern "C" {
@@ -884,6 +940,30 @@ int dfx_link_state_backward(const dfx_pack_t* p, int n, const float* q, const fl
     memset(&la, 0, sizeof la);
     la.q = q; la.qd = qd; la.g_X_sc = g_X_sc; la.g_X_sm = g_X_sm; la.g_v_s = g_v_s; la.gq = gq; la.gqd = gqd;
     return run_link_state(p, n, la, true, stream);
+}
+
+int dfx_contact_state_forward(const dfx_pack_t* p, int n, const float* q, const float* qd,
+                              float* contact_f, float* contact_height, float* body_f_contact, void* stream) {
+    if (!p || n <= 0 || !q || !qd) return (int)cudaErrorInvalidValue;
+    if (!contact_f && !contact_height && !body_f_contact) return 0;
+    ContactStateArgs ca;
+    memset(&ca, 0, sizeof ca);
+    ca.q = q; ca.qd = qd; ca.corder = p->d_corder;
+    ca.contact_f = contact_f; ca.contact_height = contact_height; ca.body_f = body_f_contact;
+    return run_contact_state(p, n, ca, false, stream);
+}
+
+int dfx_contact_state_backward(const dfx_pack_t* p, int n, const float* q, const float* qd,
+                               const float* g_contact_f, const float* g_contact_height, const float* g_body_f_contact,
+                               float* gq, float* gqd, void* stream) {
+    if (!p || n <= 0 || !q || !qd) return (int)cudaErrorInvalidValue;
+    if (!gq && !gqd) return 0;
+    ContactStateArgs ca;
+    memset(&ca, 0, sizeof ca);
+    ca.q = q; ca.qd = qd; ca.corder = p->d_corder;
+    ca.g_contact_f = g_contact_f; ca.g_contact_height = g_contact_height; ca.g_body_f = g_body_f_contact;
+    ca.gq = gq; ca.gqd = gqd;
+    return run_contact_state(p, n, ca, true, stream);
 }
 
 }  // extern "C"

@@ -81,8 +81,10 @@ struct DfxTileApi {
     size_t (*smem)(const void* kernel_args, int backward);   // dynamic shared memory (bytes); backward: bit 0 adjoint, bit 1 wrench
     int (*launch)(void* kernel_args, int backward, int wrench, void* stream);   // wrench != 0: the external-wrench kernels
     int (*launch_recompute)(void* kernel_args, int wrench, void* stream);       // forward into the workspace + adjoint, one launch
-    int (*launch_link_state)(void* kernel_args, const void* link_args, int backward, void* stream);   // link_args: a LinkStateArgs
+    // a readout of (q, qd) -- op: DfxReadout; args: its LinkStateArgs or ContactStateArgs
+    int (*launch_readout)(void* kernel_args, int op, const void* args, int backward, void* stream);
 };
+enum DfxReadout { kReadoutLinkState = 0, kReadoutContactState = 1 };
 const DfxTileApi* dfx_tile_api_e8(void);
 const DfxTileApi* dfx_tile_api_e16(void);
 const DfxTileApi* dfx_tile_api_e32(void);

@@ -21,6 +21,7 @@ struct PackHost {
     // offsets into ints / floats, in the order of the pointer fields of Pack
     std::vector<size_t> int_off, float_off;
     Pack header;  // scalar fields filled; pointer fields filled by bind()
+    std::vector<int> corder;   // (C) Model index of the pack's contact n (not staged: read by the contact state only)
     Layout layout;       // forward kernels (legacy mode: also the backward kernels)
     Layout layout_bwd;   // backward kernels
     int layout_mode = kLayoutLegacy;
@@ -299,6 +300,7 @@ inline bool build_pack(const DfxModelDesc& d, PackHost& out, std::string& err) {
     push_f(vec(d.joint_armature, D));
     push_f(cpoint); push_f(cdist); push_f(cmat);
     push_f(vec(d.muscle_points, W * 3));
+    out.corder = corder;
     out.set_layout_mode(kLayoutLegacy);
     return true;
 }

@@ -273,4 +273,155 @@ DFX_HD void link_state_backward(const Pack& P, const Layout& Y, SP s, const Grp&
     if (a.gqd) DFX_FOR(i, D) a.gqd[(long long)env * D + i] = s[Y.aqd + i];
 }
 
+// ---- contact state of (q, qd) (include/dfx.h dfx_contact_state_forward / _backward): the step's ground-contact model
+// (contact_point_fwd) at the state, as the first substep of an env-step from it applies it.  Per point k, in the Model's contact
+// order: the force the ground exerts on the link, -ftot (ftot is what the step adds to body_f_s, where it acts like gravity:
+// f = f_b - (...)), and the height c of the point above the plane; per link, the sum (tau, F) of its points' forces, tau about
+// the link's centre of mass (the DfxExternalWrench convention).  One item per link walks its points in pack order (cbody_start),
+// so every sum is in a fixed order, with no atomics.
+struct ContactStateArgs {
+    const float* q; const float* qd;
+    const int* corder;                                          // [C]: Model index of the pack's contact n (dfx_pack_create)
+    float* contact_f; float* contact_height; float* body_f;     // forward outputs [N, C, 3], [N, C], [N, L, 6] (NULL: skip)
+    const float* g_contact_f; const float* g_contact_height; const float* g_body_f;   // backward: their cotangents (NULL == 0)
+    float* gq; float* gqd;                                      // backward outputs [N, Q], [N, D] (NULL: skip)
+};
+
+template <class Grp>
+DFX_HD void contact_state_kinematics(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const ContactStateArgs& a) {
+    LinkStateArgs la{};
+    la.q = a.q; la.qd = a.qd;
+    link_state_kinematics(P, Y, s, g, env, la);
+}
+
+// contact point k (pack order) on link b: the point p after the contact_dist shift, where the step applies the force
+DFX_HD V3 contact_point_world(const Pack& P, const Layout& Y, SP s, int b, int k) {
+    V3 p = xf_point(ld7(s + Y.Xsc + b * 7), ld3(P.cpoint + k * 3));
+    p.y -= P.cdist[k];
+    return p;
+}
+
+template <class Grp>
+DFX_HD void contact_state_forward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const ContactStateArgs& a) {
+    const int L = P.L, C = P.C;
+    contact_state_kinematics(P, Y, s, g, env, a);
+    DFX_FOR(i, L) {
+        const V3 cm = ld3(s + Y.Xsm + i * 7);
+        V3 F = v3zero(), tau = v3zero();
+        for (int k = P.cbody_start[i]; k < P.cbody_start[i + 1]; ++k) {
+            const long long o = (long long)env * C + a.corder[k];
+            const V3 p = contact_point_world(P, Y, s, i, k);
+            const V3 f = P.ground ? v3zero() - contact_point_fwd(P, Y, s, k).v : v3zero();
+            if (a.contact_f) st3(a.contact_f + o * 3, f);
+            if (a.contact_height) a.contact_height[o] = p.y;
+            F += f;
+            tau += cross(p - cm, f);
+        }
+        if (a.body_f) {
+            float* w = a.body_f + ((long long)env * L + i) * 6;
+            st3(w, tau);
+            st3(w + 3, F);
+        }
+    }
+}
+
+// Adjoint of the force model of one penetrating point: the cotangent aftot of ftot -> those of p (ap) and dp/dt (adpdt).  This
+// restates the part of contact_point_adj (dfx_phases.h) after its torque term, which it must mirror line for line: that
+// function stays as it is so that the step kernels keep their code.
+DFX_HD void contact_force_adj(V3 p, V3 dpdt, float ke, float kd, float kf, float mu, V3 aftot, V3& ap, V3& adpdt) {
+    const float c = p.y;
+    const float vn = dpdt.y;
+    const V3 vt = V3{dpdt.x, 0.0f, dpdt.z};
+    const float mn = fminf(vn, 0.0f);
+    const float len = sqrtf(dot(vt, vt));
+    const V3 nvt = len > 0.0f ? V3{vt.x / len, vt.y / len, vt.z / len} : v3zero();
+    const float A = kf * len, Bc = 0.0f - mu * c * ke;
+    const float cap = fminf(A, Bc);
+    const float a_nf = aftot.y;  // d/d(fn+fd)
+    const V3 aft = aftot;
+    // ft = nvt * cap
+    const V3 anvt = aft * cap;
+    const float acap = dot(nvt, aft);
+    float ac = 0.0f, alen = 0.0f;
+    if (A < Bc) alen += kf * acap; else ac += -mu * ke * acap;
+    V3 avt = nvt * alen;
+    if (len > 0.0f) {
+        const float inv = 1.0f / len;
+        avt += (anvt - nvt * dot(nvt, anvt)) * inv;
+    }
+    // fd = min(vn,0) * kd * (-c)
+    float avn = 0.0f;
+    if (vn < 0.0f) avn += kd * (0.0f - c) * a_nf;
+    ac += -(mn * kd) * a_nf;
+    // fn = c ke
+    ac += ke * a_nf;
+    // vt = dpdt - n vn ; vn = dpdt.y
+    adpdt = avt;
+    avn -= avt.y;
+    adpdt.y += avn;
+    ap.y += ac;
+}
+
+// adjoint: the kinematics recomputed from (q, qd); per link item, its points' cotangents (height: every point; force: penetrating
+// points with the ground on) added into aXsc, av and aXsm (the centre of mass of the torque) of that link, in pack order, then A1
+// and the rest of the kinematics adjoint, as link_state_backward
+template <class Grp>
+DFX_HD void contact_state_backward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const ContactStateArgs& a) {
+    const int L = P.L, C = P.C, Q = P.Q, D = P.D;
+    contact_state_kinematics(P, Y, s, g, env, a);
+    DFX_FOR(i, L * 7) s[Y.aXsc + i] = 0.0f;
+    DFX_FOR(i, L * 7) s[Y.aXsm + i] = 0.0f;
+    DFX_FOR(i, L * 6) s[Y.av + i] = 0.0f;
+    DFX_FOR(i, L * 6) s[Y.aa + i] = 0.0f;
+    DFX_FOR(i, D * 6) s[Y.aS + i] = 0.0f;
+    DFX_FOR(i, Q) s[Y.aq + i] = 0.0f;
+    DFX_FOR(i, D) s[Y.aqd + i] = 0.0f;
+    g.sync();
+    DFX_FOR(i, L) {
+        const Xf X = ld7(s + Y.Xsc + i * 7);
+        const SV vs = ld6(s + Y.v + i * 6);
+        const V3 cm = ld3(s + Y.Xsm + i * 7);
+        const V3 gtau = a.g_body_f ? ld3(a.g_body_f + ((long long)env * L + i) * 6) : v3zero();
+        const V3 gF = a.g_body_f ? ld3(a.g_body_f + ((long long)env * L + i) * 6 + 3) : v3zero();
+        V3 acm = v3zero();
+        for (int k = P.cbody_start[i]; k < P.cbody_start[i + 1]; ++k) {
+            const long long o = (long long)env * C + a.corder[k];
+            const V3 pt = ld3(P.cpoint + k * 3);
+            const V3 p = contact_point_world(P, Y, s, i, k);
+            V3 ap = v3zero(), aw = v3zero(), adpdt = v3zero();
+            if (a.g_contact_height) ap.y += a.g_contact_height[o];
+            if (P.ground && !(p.y >= 0.0f)) {       // (a NaN height takes this branch, as in contact_point_adj)
+                const V3 f = v3zero() - contact_point_fwd(P, Y, s, k).v;
+                // loss terms g_f . f + gF . f + gtau . ((p - cm) x f)
+                V3 af = gF, ar = v3zero();
+                if (a.g_contact_f) af += ld3(a.g_contact_f + o * 3);
+                cross_adj(p - cm, f, gtau, ar, af);
+                ap += ar;
+                acm -= ar;
+                const float ke = P.cmat[k * 4 + 0], kd = P.cmat[k * 4 + 1], kf = P.cmat[k * 4 + 2], mu = P.cmat[k * 4 + 3];
+                contact_force_adj(p, vs.v + cross(vs.w, p), ke, kd, kf, mu, v3zero() - af, ap, adpdt);
+                // dpdt = v + w x p
+                cross_adj(vs.w, p, adpdt, aw, ap);
+            }
+            // p = X.p + R(X.q) pt - n d
+            const Q4 aq = qrot_adj_q(X.q, pt, ap);
+            const SP ax = s + Y.aXsc + i * 7;
+            const SP avp = s + Y.av + i * 6;
+            const float c7[7] = {ap.x, ap.y, ap.z, aq.x, aq.y, aq.z, aq.w};
+            const float c6[6] = {aw.x, aw.y, aw.z, adpdt.x, adpdt.y, adpdt.z};
+#pragma unroll
+            for (int c = 0; c < 7; ++c) ax[c] += c7[c];
+#pragma unroll
+            for (int c = 0; c < 6; ++c) avp[c] += c6[c];
+        }
+        add3(s + Y.aXsm + i * 7, acm);
+        kin_adj_local(P, Y, s, i);
+    }
+    g.sync();
+    kin_adj(P, Y, s, g);
+    g.sync();
+    if (a.gq) DFX_FOR(i, Q) a.gq[(long long)env * Q + i] = s[Y.aq + i];
+    if (a.gqd) DFX_FOR(i, D) a.gqd[(long long)env * D + i] = s[Y.aqd + i];
+}
+
 }  // namespace dfx

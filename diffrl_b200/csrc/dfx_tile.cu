@@ -444,6 +444,43 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_link_state_kernel(cons
     else link_state_forward(P, Y, s, g, env, la);
 }
 
+// Contact state (include/dfx.h dfx_contact_state_forward / _backward; dfx_step.h contact_state_*): the set-up of
+// dfx_tile_link_state_kernel line for line (keep the two in step), then the ground-contact model at (q, qd) or its adjoint.
+template <int NW, int MINB, bool BACKWARD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_contact_state_kernel(const __grid_constant__ KernelArgs ka,
+                                                                              const __grid_constant__ ContactStateArgs ca) {
+    constexpr int E = DFX_TILE_E;
+    extern __shared__ __align__(128) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += NW * 32) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += NW * 32) ipack[i] = ka.blob.ints[i];
+    int* cta_area = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    if (threadIdx.x < 4) cta_area[threadIdx.x] = 0;
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+    P.jmask = tile_joint_mask(SL, SD, SQ, SC, SM);
+    constexpr Layout Y = make_layout(SL, SD, SQ, SC, SM, MODE, BACKWARD);
+
+    GroupTile<NW, E, PATH> g;
+    const int lane32 = threadIdx.x & 31;
+    g.lane = (threadIdx.x >> 5) * (32 / E) + lane32 / E;
+    g.e = lane32 % E;
+    g.tile = blockIdx.x;
+    g.ntiles = gridDim.x;
+    g.task_count = cta_area;
+    g.task_list = cta_area + 8;
+    g.mbar = nullptr;
+    g.par0 = g.par1 = 0u;
+    g.tile_base = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    int env = blockIdx.x * E + g.e;          // (lanes past the end redo the last environment, as in dfx_tile_kernel)
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const SP s{g.tile_base + g.e};
+    if (BACKWARD) contact_state_backward(P, Y, s, g, env, ca);
+    else contact_state_forward(P, Y, s, g, env, ca);
+}
+
 // 128-byte aligned offsets so that the bulk copies of the tile stay 16-byte aligned
 static int tile_pack_floats(const KernelArgs& ka) {
     const int bytes = (((ka.blob.n_floats + 3) & ~3) + ((ka.blob.n_ints + 3) & ~3)) * 4;
@@ -474,12 +511,12 @@ static cudaError_t tile_launch(void (*kern)(P...), const Layout& Y, int per_env,
 }
 
 // what a tile entry point asks of the articulation's model entry (below): its layout mode, or a launch of one of its kernels
-enum class TileOp { mode, step, recompute, link_state };
+enum class TileOp { mode, step, recompute, link_state, contact_state };
 struct TileCall {
     TileOp op;
     bool backward, wrench;
     KernelArgs* ka;
-    const LinkStateArgs* la;
+    const void* ra;         // the readout's kernel parameter: a LinkStateArgs (link_state) or a ContactStateArgs (contact_state)
     cudaStream_t stream;
 };
 
@@ -493,8 +530,8 @@ static int tile_model(const TileCall& c) {
     constexpr Layout YF = make_layout(SL, SD, SQ, SC, SM, LM, false), YB = make_layout(SL, SD, SQ, SC, SM, LM, true);
     const int per_f = scratch_floats(YF, SL, false, c.wrench), per_b = scratch_floats(YB, SL, true, c.wrench);
     KernelArgs& ka = *c.ka;
-    // (kernels referenced in the order of the step, its external-wrench twin, the recompute adjoint, the link state: nvcc emits
-    //  the kernels in the order they are first referenced, and the code of some depends on that order)
+    // (kernels referenced in the order of the step, its external-wrench twin, the recompute adjoint, the link state, the contact
+    //  state: nvcc emits the kernels in the order they are first referenced, and the code of some depends on that order)
     if (c.op == TileOp::step && !c.wrench)
         return c.backward ? tile_launch<NWB>(dfx_tile_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream)
                           : tile_launch<NWF>(dfx_tile_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream);
@@ -505,8 +542,14 @@ static int tile_model(const TileCall& c) {
         if (c.op == TileOp::recompute)
             return c.wrench ? tile_launch<NWB>(dfx_tile_recompute_wrench_kernel<NWB, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YB, dfx_max(per_f, per_b), ka, c.stream)
                             : tile_launch<NWB>(dfx_tile_recompute_kernel<NWB, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YB, dfx_max(per_f, per_b), ka, c.stream);
-        return c.backward ? tile_launch<NWB>(dfx_tile_link_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, *c.la)
-                          : tile_launch<NWF>(dfx_tile_link_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, *c.la);
+        if (c.op == TileOp::link_state) {
+            const LinkStateArgs& la = *static_cast<const LinkStateArgs*>(c.ra);
+            return c.backward ? tile_launch<NWB>(dfx_tile_link_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, la)
+                              : tile_launch<NWF>(dfx_tile_link_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, la);
+        }
+        const ContactStateArgs& ca = *static_cast<const ContactStateArgs*>(c.ra);
+        return c.backward ? tile_launch<NWB>(dfx_tile_contact_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, ca)
+                          : tile_launch<NWF>(dfx_tile_contact_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, ca);
     }
     return -1;      // (the A/B variants are asked for the step only)
 }
@@ -604,14 +647,15 @@ static int tile_launch_recompute(void* kargs, int wrench, void* stream) {
     return tile_run(TileCall{TileOp::recompute, true, wrench != 0, static_cast<KernelArgs*>(kargs), nullptr, static_cast<cudaStream_t>(stream)}, false);
 }
 
-// the link state (dfx_tile_link_state_kernel) with the step kernels' warps and occupancy.  The flag-64 (A/B) variants have none:
-// they run these, which is valid because the link state has no tape layout to match.
-static int tile_launch_link_state(void* kargs, const void* largs, int backward, void* stream) {
-    return tile_run(TileCall{TileOp::link_state, backward != 0, false, static_cast<KernelArgs*>(kargs), static_cast<const LinkStateArgs*>(largs),
-                             static_cast<cudaStream_t>(stream)}, false);
+// a readout of (q, qd) -- op kReadoutLinkState: the link state (dfx_tile_link_state_kernel), kReadoutContactState: the contact state
+// (dfx_tile_contact_state_kernel) -- with the step kernels' warps and occupancy.  The flag-64 (A/B) variants have none: they run
+// these, which is valid because a readout has no tape layout to match.
+static int tile_launch_readout(void* kargs, int op, const void* args, int backward, void* stream) {
+    const TileOp top = op == kReadoutContactState ? TileOp::contact_state : TileOp::link_state;
+    return tile_run(TileCall{top, backward != 0, false, static_cast<KernelArgs*>(kargs), args, static_cast<cudaStream_t>(stream)}, false);
 }
 
 const DfxTileApi* DFX_TILE_FN(dfx_tile_api)(void) {
-    static const DfxTileApi api = {tile_mode, tile_smem, tile_launch_step, tile_launch_recompute, tile_launch_link_state};
+    static const DfxTileApi api = {tile_mode, tile_smem, tile_launch_step, tile_launch_recompute, tile_launch_readout};
     return &api;
 }

@@ -80,6 +80,7 @@ def check_link_input(engine, name, t, shapes):
 
 
 LINK_STATE_FIELDS = ("body_X_sc", "body_X_sm", "body_v_s")
+CONTACT_STATE_FIELDS = ("contact_f", "contact_height", "body_f_contact")
 
 
 def wrench_struct(f_ext, g_f_ext=None):
@@ -361,6 +362,49 @@ class ArticulationEngine:
         _capi.check(code, "dfx_link_state_backward")
         return gq, gqd
 
+    def _contact_state_inputs(self, q, qd):
+        if not hasattr(self.lib, "dfx_contact_state_forward"):
+            raise _capi.DfxError("%s has no contact-state entries (dfx_contact_state_*)" % _capi.LIB_PATH)
+        q = check_link_input(self, "q", q, ((self.N * self.Q,), (self.N, self.Q)))
+        qd = check_link_input(self, "qd", qd, ((self.N * self.D,), (self.N, self.D)))
+        return q, qd
+
+    def _contact_shapes(self):
+        N, C, L = self.N, self.C, self.L
+        return {"contact_f": ((N, C, 3), (N * C, 3), (N * C * 3,)), "contact_height": ((N, C), (N * C,)),
+                "body_f_contact": ((N, L, 6), (N * L, 6), (N * L * 6,))}
+
+    def contact_state(self, q, qd, want=CONTACT_STATE_FIELDS):
+        """(contact_f [N, C, 3], contact_height [N, C], body_f_contact [N, L, 6]) of the state (q, qd) -- ``dfx_contact_state_forward``:
+        the force the ground exerts on the link at each contact point (Model contact order; zero when the point does not
+        penetrate or the ground is off), the point's signed height above the plane (negative: penetrating), and per link the
+        wrench (torque about the centre of mass, force) of its points in world axes -- the ``f_ext`` convention.  The fields not in
+        ``want`` are None (not computed).  q [N*Q] or [N, Q], qd [N*D] or [N, D], fp32 on the engine's device (ValueError
+        otherwise)."""
+        q, qd = self._contact_state_inputs(q, qd)
+        shapes = self._contact_shapes()
+        out = tuple(torch.empty(shapes[name][0], dtype=torch.float32, device=self.device) if name in want else None
+                    for name in CONTACT_STATE_FIELDS)
+        with torch.cuda.device(self.device):
+            code = self.lib.dfx_contact_state_forward(self.pack, self.N, _ptr(q), _ptr(qd), *(_ptr(o) for o in out), self._stream())
+        _capi.check(code, "dfx_contact_state_forward")
+        return out
+
+    def contact_state_backward(self, q, qd, g_contact_f, g_contact_height, g_body_f_contact, need=(True, True)):
+        """Cotangents (gq [N*Q], gqd [N*D]) of the state from those of (contact_f, contact_height, body_f_contact) (None: zero) --
+        ``dfx_contact_state_backward``, which recomputes the kinematics of (q, qd).  An output not in ``need`` is None."""
+        q, qd = self._contact_state_inputs(q, qd)
+        shapes = self._contact_shapes()
+        g = [check_link_input(self, "g_" + name, t, shapes[name])
+             for name, t in zip(CONTACT_STATE_FIELDS, (g_contact_f, g_contact_height, g_body_f_contact))]
+        gq = torch.empty(self.N * self.Q, dtype=torch.float32, device=self.device) if need[0] else None
+        gqd = torch.empty(self.N * self.D, dtype=torch.float32, device=self.device) if need[1] else None
+        with torch.cuda.device(self.device):
+            code = self.lib.dfx_contact_state_backward(self.pack, self.N, _ptr(q), _ptr(qd), *(_ptr(x) for x in g), _ptr(gq), _ptr(gqd),
+                                                       self._stream())
+        _capi.check(code, "dfx_contact_state_backward")
+        return gq, gqd
+
 
 class MappedSimStepFunction(torch.autograd.Function):
     """(q, qd, raw policy output) -> (q', qd', used): the env-step with the action map folded into the simulation launch
@@ -459,6 +503,29 @@ class LinkStateFunction(torch.autograd.Function):
         dev = ctx.engine.device
         g = [None if x is None else _f32c(x, dev) for x in (g_X_sc, g_X_sm, g_v_s)]
         gq, gqd = ctx.engine.link_state_backward(q, qd, *g, need=tuple(ctx.needs_input_grad[1:3]))
+        return None, None if gq is None else gq.view(ctx.shapes[0]), None if gqd is None else gqd.view(ctx.shapes[1])
+
+
+class ContactStateFunction(torch.autograd.Function):
+    """(q, qd) -> (contact_f [N, C, 3], contact_height [N, C], body_f_contact [N, L, 6]): what the ground does to the links
+    (``ArticulationEngine.contact_state``).  Saves only (q, qd): the backward recomputes the kinematics, so it is the same in
+    "tape" and "recompute" adjoint mode."""
+
+    @staticmethod
+    def forward(ctx, engine, q, qd):
+        qc, qdc = engine._contact_state_inputs(q, qd)
+        out = engine.contact_state(qc, qdc)
+        ctx.engine, ctx.shapes = engine, (q.shape, qd.shape)
+        ctx.set_materialize_grads(False)      # a missing cotangent is NULL for dfx_contact_state_backward, not a zero fill
+        ctx.save_for_backward(qc, qdc)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_f, g_h, g_body):
+        q, qd = ctx.saved_tensors
+        dev = ctx.engine.device
+        g = [None if x is None else _f32c(x, dev) for x in (g_f, g_h, g_body)]
+        gq, gqd = ctx.engine.contact_state_backward(q, qd, *g, need=tuple(ctx.needs_input_grad[1:3]))
         return None, None if gq is None else gq.view(ctx.shapes[0]), None if gqd is None else gqd.view(ctx.shapes[1])
 
 

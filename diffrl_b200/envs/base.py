@@ -152,6 +152,13 @@ class DFlexEnv:
         from .. import link_state
         return link_state(self.model, self.state.joint_q, self.state.joint_qd)
 
+    def contact_state(self):
+        """``diffrl_b200.contact_state`` of ``self.state``, the state the next step starts from: ``ContactState(contact_f,
+        contact_height, body_f_contact)``, [num_envs, C, 3], [num_envs, C], [num_envs, L, 6].  Differentiable: its gradient reaches
+        the actions and the start state through whichever step op produced ``self.state``."""
+        from .. import contact_state
+        return contact_state(self.model, self.state.joint_q, self.state.joint_qd)
+
     def _attach_wrench(self, state):
         """The step reads the wrench from its input State (``body_f_ext``)."""
         if self.external_wrench is None:

@@ -385,6 +385,31 @@ int dfx_link_state_backward(const dfx_pack_t* pack, int n, const float* q, const
                             const float* g_X_sc, const float* g_X_sm, const float* g_v_s,
                             float* gq, float* gqd, void* stream);
 
+/* ---- contact state: what the ground does to the links at (q, qd), differentiable -- the step's penalty ground-contact model
+ * (reference eval_rigid_contacts_art sim.py:1137) evaluated at the given state, which is exactly what the first substep of an
+ * env-step from it applies.  All fp32, world axes, env-major:
+ *   contact_f       [n*C*3]  force the ground exerts on the link at contact point k, in the Model's contact order (Model.collide,
+ *                            contact_body0); zero for a point that does not penetrate, and for every point when the ground is off
+ *                            (dfx_pack_set_gravity);
+ *   contact_height  [n*C]    signed height of point k above the plane, (X_sc p0).y - contact_dist: negative when penetrating (the c
+ *                            of the contact model), computed whether the ground is on or not;
+ *   body_f_contact  [n*L*6]  per link, (tau, F) summed over its points: F = sum f_k, tau = sum (p_k - X_sm.p) x f_k, p_k the point
+ *                            after the contact_dist shift (where the step applies it) -- the DfxExternalWrench convention, so it can
+ *                            be passed back as f_ext unchanged.
+ * Sign: inside the step the contact model's ftot is added into body_f_s, where it acts like the gravity and external terms that
+ * f = f_b - (...) subtracts, so the physical force on the link is -ftot (upward when penetrating): that is what contact_f holds.
+ * The backward recomputes the kinematics from (q, qd) and keeps nothing between the calls; the force's cotangent reaches (q, qd)
+ * only through penetrating points, the height's through every point.  Both run on the kernels dfx_link_state_* use; every sum is
+ * taken in a fixed order by one thread, so both are bit-reproducible.  With C == 0 the kernels still run when there is an output:
+ * body_f_contact and the gradients are written as zero.  Stream-ordered, no host synchronisation. */
+/* contact forces / heights / link wrenches of (q, qd); any output NULL: skip (all NULL: no launch, returns 0) */
+int dfx_contact_state_forward(const dfx_pack_t* pack, int n, const float* q, const float* qd,
+                              float* contact_f, float* contact_height, float* body_f_contact, void* stream);
+/* cotangents (NULL == 0) -> gq [n*Q], gqd [n*D] (overwritten; NULL: skip; both NULL: no launch, returns 0) */
+int dfx_contact_state_backward(const dfx_pack_t* pack, int n, const float* q, const float* qd,
+                               const float* g_contact_f, const float* g_contact_height, const float* g_body_f_contact,
+                               float* gq, float* gqd, void* stream);
+
 /* Launch configuration knob: lanes cooperating on one environment (8, 16 or 32; 0 = auto). */
 int dfx_set_group_size(int lanes);
 /* Tuning flags (default 9; for A/B timing and tests).  Lane-group kernels: bit 1 (2) = extra CTA-wide barriers between
