@@ -75,3 +75,34 @@ def contact_state(model, joint_q, joint_qd):
 
 
 ContactState = collections.namedtuple("ContactState", ["contact_f", "contact_height", "body_f_contact"])
+
+
+def dynamics_state(model, joint_q, joint_qd, joint_act=None, muscle_activation=None, f_ext=None):
+    """What the dynamics of the state (joint_q, joint_qd) of ``model``'s N environments produce under the actuation (joint_act,
+    muscle_activation) and the external link wrench f_ext, differentiable: ``DynamicsState(joint_qdd, joint_tau, H)``, fp32, in
+    the Model's dof order --
+
+    - ``joint_tau`` [N, D]: the generalized joint force, the right-hand side of the solve: -S^T f of each joint's subtree
+      (gravity, Coriolis and centrifugal terms, ground contacts, muscles, the external wrench), plus the PD drive to the joint
+      target, plus joint_act, plus the joint-limit spring and damper (-f for a free joint).  It is NOT the actuator effort alone;
+    - ``H`` [N, D, D]: the joint-space inertia J^T M J, symmetric, without the armature;
+    - ``joint_qdd`` [N, D]: the joint accelerations (H + diag(armature))^-1 joint_tau.
+
+    This is what the first substep of an env-step from the state computes before it integrates (H is built from joint_q).  One
+    kernel launch forward (include/dfx.h dfx_dynamics_state_forward) and one backward on the tile kernels (two on the lane-group
+    kernels), which re-runs a one-substep env-step into a workspace: nothing but the inputs is kept.  Gradients reach joint_q,
+    joint_qd, joint_act, muscle_activation and f_ext; only the symmetric part of H's cotangent matters.  joint_act None is zero;
+    muscle_activation None is zero (a model with muscles); f_ext [N, L, 6] in the ``DFlexEnv.set_external_wrench`` convention or
+    None.  fp32 on the model's device (ValueError otherwise)."""
+    import torch
+    from .dflex_api.sim import _engine_for
+    from .engine import DynamicsStateFunction
+    engine = _engine_for(model)
+    if joint_act is None:
+        joint_act = torch.zeros(engine.N * engine.D, dtype=torch.float32, device=engine.device)
+    if muscle_activation is None and engine.M:
+        muscle_activation = torch.zeros(engine.N * engine.M, dtype=torch.float32, device=engine.device)
+    return DynamicsState(*DynamicsStateFunction.apply(engine, joint_q, joint_qd, joint_act, muscle_activation, f_ext))
+
+
+DynamicsState = collections.namedtuple("DynamicsState", ["joint_qdd", "joint_tau", "H"])

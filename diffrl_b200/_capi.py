@@ -75,6 +75,11 @@ def lib():
     if hasattr(L, "dfx_contact_state_forward"):    # contact state of (q, qd) (include/dfx.h dfx_contact_state_*)
         L.dfx_contact_state_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, ctypes.c_void_p]
         L.dfx_contact_state_backward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, _F, _F, ctypes.c_void_p]
+    if hasattr(L, "dfx_dynamics_state_forward"):    # dynamics state of (q, qd, act, musc, f_ext) (include/dfx.h dfx_dynamics_state_*)
+        L.dfx_dynamics_workspace_floats.restype = ctypes.c_longlong
+        L.dfx_dynamics_workspace_floats.argtypes = [ctypes.c_void_p, ctypes.c_int]
+        L.dfx_dynamics_state_forward.argtypes = [ctypes.c_void_p, ctypes.c_int] + [_F] * 8 + [ctypes.c_void_p]
+        L.dfx_dynamics_state_backward.argtypes = [ctypes.c_void_p, ctypes.c_int] + [_F] * 14 + [ctypes.c_void_p]
     if os.environ.get("DFX_FLAGS"):      # tuning flags of include/dfx.h (A/B runs of the test-suite)
         L.dfx_set_flags(int(os.environ["DFX_FLAGS"]))
     _lib = L

@@ -284,6 +284,45 @@ __global__ void __launch_bounds__(kMaxThreads) dfx_contact_state_kernel(const __
     else contact_state_forward(P, Y, s, g, env, ca);
 }
 
+// Dynamics state (include/dfx.h dfx_dynamics_state_forward / _backward; dfx_step.h dynamics_state_*): the set-up of
+// dfx_link_state_kernel line for line (keep the two in step), then the first substep's dynamics, or their seeded adjoint on the
+// one-substep tape that dfx_step_forward_ex wrote into the workspace (ka.step.tape_in) in the launch before.
+template <int G, bool BACKWARD, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(kMaxThreads) dfx_dynamics_state_kernel(const __grid_constant__ KernelArgs ka,
+                                                                       const __grid_constant__ DynamicsStateArgs da) {
+    extern __shared__ __align__(16) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += blockDim.x) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += blockDim.x) ipack[i] = ka.blob.ints[i];
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    Layout Y = ka.layout;
+    if constexpr (SL > 0) {
+        P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+        constexpr Layout kY = make_layout(SL, SD, SQ, SC, SM);
+        Y = kY;
+    }
+    const int kEnvsPerCta = blockDim.x / G;
+    const int local = threadIdx.x / G;
+    int env = blockIdx.x * kEnvsPerCta + local;      // (groups past the end redo the last environment, as in step_kernel_body)
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const int lane_in_warp = threadIdx.x & 31;
+    GroupCuda<G> g;
+    g.lane = threadIdx.x % G;
+    g.psync = (ka.step.flags & 2) != 0;
+    g.mask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << ((lane_in_warp / G) * G));
+    float* s = smem + ka.pack_smem_floats + ka.cta_area_floats + (size_t)local * ka.scratch_stride;
+    g.scratch0 = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    g.task_count = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    g.task_list = g.task_count + 4;
+    g.stride = ka.scratch_stride;
+    g.envs_shift = 31 - __clz(kEnvsPerCta > 0 ? kEnvsPerCta : 1);
+    g.cta_mode = (ka.step.flags & 8) != 0;
+    if (BACKWARD) dynamics_state_backward(P, Y, s, g, env, ka.step, da);
+    else dynamics_state_forward(P, Y, s, g, env, da);
+}
+
 }  // namespace dfx
 
 // =====================================================================================
@@ -492,14 +531,15 @@ static int counted(int e) {
 }
 
 // the lane-group kernel families
-enum GroupFamily { kStep, kStepWrench, kLinkState, kContactState };
+enum GroupFamily { kStep, kStepWrench, kLinkState, kContactState, kDynamicsState };
 
 // one lane-group launch: the family's kernel of group width G, size-specialised (SL..SM > 0) or generic, with plan_launch's
-// geometry; ra: the readout's kernel parameter (a LinkStateArgs or a ContactStateArgs), NULL for the step families
+// geometry; ra: the readout's kernel parameter (a LinkStateArgs, ContactStateArgs or DynamicsStateArgs), NULL for the step
+// families.  The external-wrench step and the dynamics state keep the wrench past the layout's end.
 template <GroupFamily F, int G, bool BWD, int SL, int SD, int SQ, int SC, int SM>
 static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const void* ra, cudaStream_t stream) {
     ka.layout = BWD ? p->host.layout_bwd : p->host.layout;
-    const LaunchPlan lp = plan_launch(p, G, BWD, F == kStepWrench);
+    const LaunchPlan lp = plan_launch(p, G, BWD, F == kStepWrench || F == kDynamicsState);
     ka.scratch_stride = lp.scratch_stride;
     ka.pack_smem_floats = lp.pack_bytes / 4;
     ka.cta_area_floats = lp.cta_area_bytes / 4;
@@ -517,6 +557,8 @@ static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const void* ra
         return go(dfx_link_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *static_cast<const LinkStateArgs*>(ra));
     } else if constexpr (F == kContactState) {
         return go(dfx_contact_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *static_cast<const ContactStateArgs*>(ra));
+    } else if constexpr (F == kDynamicsState) {
+        return go(dfx_dynamics_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *static_cast<const DynamicsStateArgs*>(ra));
     } else {
         // (the step kernel is referenced before its external-wrench twin, in every instantiation: nvcc emits the kernels in the
         //  order they are first referenced, and the code of some depends on that order)
@@ -677,6 +719,36 @@ static int run_contact_state(const dfx_pack_t* p, int n, const ContactStateArgs&
     KernelArgs ka = kernel_args(p, a, nullptr);
     if (p->tile) return counted(tile_api(p->tile)->launch_readout(&ka, kReadoutContactState, &ca, backward, stream));
     return run_group<kContactState>(p, ka, backward, &ca, (cudaStream_t)stream);
+}
+
+// ---- dynamics state (include/dfx.h dfx_dynamics_state_*): on the kernels run_link_state picks.  The backward first runs a
+// one-substep env-step (substeps = mm_freq = 1, dt = 0: only its tape row and H^-1 block are used) from the same inputs into the
+// workspace, with fp32 rows whatever dfx_set_tape_dtype says -- inside the adjoint's launch on the tile kernels, as the launch
+// before on the lane-group kernels -- then the seeded adjoint of its dynamics reads them back.
+static TapeGeom dynamics_tape(const dfx_pack_t* p, int n) {
+    return tape_geom(p->header.L, p->header.Q, p->header.D, tape_envs(p, n), 1, 1, false);
+}
+
+static int run_dynamics_state(const dfx_pack_t* p, int n, const DynamicsStateArgs& da, float* ws, bool backward, void* stream) {
+    StepArgs a{};
+    a.N = n;
+    a.flags = g_flags;
+    const DfxExternalWrench w{da.f_ext, nullptr};
+    if (backward) {
+        const TapeGeom t = dynamics_tape(p, n);
+        a.substeps = 1; a.mm_freq = 1;
+        a.q = da.q; a.qd = da.qd; a.act = da.act; a.musc = da.musc;
+        a.tape = ws; a.tape_in = ws; a.hinv_base = t.hinv_base;
+        a.q_out = ws + t.total; a.qd_out = a.q_out + (long long)n * p->header.Q;
+    }
+    KernelArgs ka = kernel_args(p, a, &w);        // (the tile backward's forward reads ka.wrench; a NULL f_ext is zero)
+    if (p->tile) return counted(tile_api(p->tile)->launch_readout(&ka, kReadoutDynamicsState, &da, backward, stream));
+    if (backward) {
+        const int e = dfx_step_forward_ex(p, n, 1, 1, 0.0, da.q, da.qd, da.act, da.musc, a.q_out, a.qd_out, ws, nullptr, stream,
+                                          da.f_ext ? &w : nullptr);
+        if (e != 0) return e;
+    }
+    return run_group<kDynamicsState>(p, ka, backward, &da, (cudaStream_t)stream);
 }
 
 extern "C" {
@@ -964,6 +1036,35 @@ int dfx_contact_state_backward(const dfx_pack_t* p, int n, const float* q, const
     ca.g_contact_f = g_contact_f; ca.g_contact_height = g_contact_height; ca.g_body_f = g_body_f_contact;
     ca.gq = gq; ca.gqd = gqd;
     return run_contact_state(p, n, ca, true, stream);
+}
+
+long long dfx_dynamics_workspace_floats(const dfx_pack_t* p, int n) {
+    if (!p || n <= 0) return -1;
+    return dynamics_tape(p, n).total + (long long)n * (p->header.Q + p->header.D);
+}
+
+int dfx_dynamics_state_forward(const dfx_pack_t* p, int n, const float* q, const float* qd, const float* act, const float* musc,
+                               const float* f_ext, float* joint_qdd, float* joint_tau, float* H, void* stream) {
+    if (!p || n <= 0 || !q || !qd || !act || (p->header.M > 0 && !musc)) return (int)cudaErrorInvalidValue;
+    if (!joint_qdd && !joint_tau && !H) return 0;
+    DynamicsStateArgs da;
+    memset(&da, 0, sizeof da);
+    da.q = q; da.qd = qd; da.act = act; da.musc = musc; da.f_ext = f_ext;
+    da.joint_qdd = joint_qdd; da.joint_tau = joint_tau; da.H = H;
+    return run_dynamics_state(p, n, da, nullptr, false, stream);
+}
+
+int dfx_dynamics_state_backward(const dfx_pack_t* p, int n, const float* q, const float* qd, const float* act, const float* musc,
+                                const float* f_ext, float* workspace, const float* g_qdd, const float* g_tau, const float* g_H,
+                                float* gq, float* gqd, float* gact, float* gmusc, float* g_f_ext, void* stream) {
+    if (!p || n <= 0 || !q || !qd || !act || (p->header.M > 0 && !musc) || !workspace) return (int)cudaErrorInvalidValue;
+    if (!gq && !gqd && !gact && !gmusc && !g_f_ext) return 0;
+    DynamicsStateArgs da;
+    memset(&da, 0, sizeof da);
+    da.q = q; da.qd = qd; da.act = act; da.musc = musc; da.f_ext = f_ext;
+    da.g_qdd = g_qdd; da.g_tau = g_tau; da.g_H = g_H;
+    da.gq = gq; da.gqd = gqd; da.gact = gact; da.gmusc = gmusc; da.g_f_ext = g_f_ext;
+    return run_dynamics_state(p, n, da, workspace, true, stream);
 }
 
 }  // extern "C"

@@ -1702,19 +1702,26 @@ DFX_HD void integrate_adj(const Pack& P, const Layout& Y, SP s, float dt, const 
 // adjoint of one substep.  Pre: scratch [q .. qdd] = the substep's taped block (entering q, qd and the
 // forward intermediates), act, musc, A = H^-1 of the segment; aq, aqd = cotangents of the substep output.  Post: aq, aqd = cotangents of the substep input;
 // aact, amusc, aH (Lm slot) accumulated.  `apply_crba` is set on the substep that built H.
-template <bool kWrench = false, class Grp>
+// kSeeded (dfx_step.h dynamics_state_backward): the adjoint of the substep's dynamics without its integrator -- integrate_adj is
+// skipped (aqdd, aq, aqd are the caller's seeds), and the cotangent gtau[D] of tau (NULL: none) joins atau after solve_adj's
+// Hs update, which reads other threads' atau entries without a barrier of its own; a barrier then precedes crba_adj / tau_adj.
+template <bool kWrench = false, bool kSeeded = false, class Grp>
 DFX_HD void substep_adj(const Pack& P, const Layout& Y, SP s, float dt, bool apply_crba, HinvView hv, const RowFmt& rf, const Grp& g,
-                        int xw = -1) {
+                        int xw = -1, const float* gtau = nullptr) {
     zero_range(s + Y.aXsc, P.L * 32 + P.D * 6, g);      // aXsc, av, aXsm, aS, aa are adjacent (af is overwritten by tau_adj)
     zero_range(s + Y.aIbar, P.L * 12, g);
     // (no barrier: integrate_adj and solve_adj do not touch the zeroed accumulators, and two barriers follow before their first use)
     // phase_sync(): CTA-wide barrier that keeps the warps of a CTA inside the same phase, so that the
     // instruction working set per SM is one or two phases instead of the whole body
-    integrate_adj(P, Y, s, dt, g);
+    if constexpr (!kSeeded) integrate_adj(P, Y, s, dt, g);
     solve_adj(P, Y, s, hv, g);              // tau slot <- atau
     g.copy_wait_all();                      // the bulk of the tape row (transforms, S, v, a, wrenches) is needed from here on
     g.row_unpack(s + Y.q, s + Y.stage, rf); // (bf16 tape: the staged halves become the fp32 scratch fields)
     g.sync();
+    if constexpr (kSeeded) {
+        if (gtau) DFX_FOR(i, P.D) s[Y.tau + i] += gtau[i];
+        g.sync();
+    }
     if (apply_crba) crba_adj(P, Y, s, g);
     tau_adj(P, Y, s, s + Y.tau, g);
     g.phase_sync();

@@ -99,7 +99,9 @@ DFX_HD void load_wrench(const Pack& P, SP s, const Grp& g, int env, const DfxExt
     DFX_FOR(i, P.L * 6) s[xw + i] = w.f_ext[(long long)env * P.L * 6 + i];
 }
 
-template <bool kWrench = false, class Grp>
+// kNullWrench (the dynamics state's one-substep forward, dfx_tile_dynamics_backward_kernel): a NULL w.f_ext reads as zero, so one
+// instantiation serves with and without a wrench; off for the step kernels, which keep their code.
+template <bool kWrench = false, bool kNullWrench = false, class Grp>
 DFX_HD void env_step_forward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const StepArgs& a,
                              const DfxExternalWrench& w = DfxExternalWrench{nullptr, nullptr}) {
     const int Q = P.Q, D = P.D, DD = D * D;
@@ -108,7 +110,11 @@ DFX_HD void env_step_forward(const Pack& P, const Layout& Y, SP s, const Grp& g,
     DFX_FOR(i, Q) s[Y.q + i] = a.q[(long long)env * Q + i];
     DFX_FOR(i, D) s[Y.qd + i] = a.qd[(long long)env * D + i];
     load_actuation(P, Y, s, g, env, a, true);
-    if constexpr (kWrench) load_wrench(P, s, g, env, w, xw);
+    if constexpr (kWrench && kNullWrench) {
+        DFX_FOR(i, P.L * 6) s[xw + i] = w.f_ext ? w.f_ext[(long long)env * P.L * 6 + i] : 0.0f;
+    } else if constexpr (kWrench) {
+        load_wrench(P, s, g, env, w, xw);
+    }
     for (int i = Y.qdd + D + g.lane; i < Y.q + Y.tape_row; i += Grp::G) s[i] = 0.0f;   // row padding
     if (g.lane == 0) s[Y.cmask] = 0.0f;
     DFX_FOR(i, P.L * 12) s[Y.fx + i] = 0.0f;   // fixed-point wrench accumulators (L x 6 low + high words)
@@ -422,6 +428,105 @@ DFX_HD void contact_state_backward(const Pack& P, const Layout& Y, SP s, const G
     g.sync();
     if (a.gq) DFX_FOR(i, Q) a.gq[(long long)env * Q + i] = s[Y.aq + i];
     if (a.gqd) DFX_FOR(i, D) a.gqd[(long long)env * D + i] = s[Y.aqd + i];
+}
+
+// ---- dynamics state of (q, qd, act, musc, f_ext) (include/dfx.h dfx_dynamics_state_forward / _backward): what the first substep
+// of an env-step from the state computes before it integrates -- the joint forces tau (the right-hand side of the solve), the
+// joint-space inertia H = J^T M J (without armature) and q'' = (H + diag(armature))^-1 tau.  The wrench is always built in
+// (f_ext NULL reads as zero), so the scratch ends past the layout's (dfx_pack.h wrench_scratch_end).
+struct DynamicsStateArgs {
+    const float* q; const float* qd; const float* act; const float* musc; const float* f_ext;   // inputs (f_ext NULL == 0)
+    float* joint_qdd; float* joint_tau; float* H;               // forward outputs [N, D], [N, D], [N, D, D] (NULL: skip)
+    const float* g_qdd; const float* g_tau; const float* g_H;   // backward: their cotangents (NULL == 0; g_H need not be symmetric)
+    float* gq; float* gqd; float* gact; float* gmusc; float* g_f_ext;   // backward outputs [N, Q / D / D / M / L*6] (NULL: skip)
+};
+
+// The first substep of env_step_forward<true> up to and including solve_fwd, phase for phase and barrier for barrier, with the
+// stores of the derived dumps (tau after tau_fwd, H after crba_fwd, q'' after solve_fwd) and no tape.  It restates that function,
+// which it must stay in step with: env_step_forward stays as it is so that the step kernels keep their code, and the readouts are
+// checked bit for bit against the derived dumps of a one-substep env-step.
+template <class Grp>
+DFX_HD void dynamics_state_forward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const DynamicsStateArgs& a) {
+    const int Q = P.Q, D = P.D, M = P.M, L = P.L, DD = D * D;
+    const int xw = wrench_offset(Y, false);
+    DFX_FOR(i, Q) s[Y.q + i] = a.q[(long long)env * Q + i];
+    DFX_FOR(i, D) s[Y.qd + i] = a.qd[(long long)env * D + i];
+    DFX_FOR(i, D) s[Y.act + i] = a.act[(long long)env * D + i];
+    DFX_FOR(i, M) s[Y.musc + i] = a.musc[(long long)env * M + i];
+    DFX_FOR(i, L * 6) s[xw + i] = a.f_ext ? a.f_ext[(long long)env * L * 6 + i] : 0.0f;
+    if (g.lane == 0) s[Y.cmask] = 0.0f;
+    DFX_FOR(i, L * 12) s[Y.fx + i] = 0.0f;   // fixed-point wrench accumulators
+    g.sync();
+    if constexpr (Grp::kFusedPhases) {
+        DFX_FOR(i, L) kin_local_fwd(P, Y, s, i);
+        g.sync();
+    }
+    kin_fwd(P, Y, s, g);
+    g.phase_sync();
+    body_and_contact_fwd<true>(P, Y, s, g, xw);
+    muscle_fwd(P, Y, s, g);
+    wrench_collect(P, Y, s, g);
+    g.phase_sync();
+    tau_fwd(P, Y, s, g);
+    g.phase_sync();
+    if (a.joint_tau) DFX_FOR(i, D) a.joint_tau[(long long)env * D + i] = s[Y.tau + i];
+    if (Y.overlay) g.sync();               // (Lm, Icmp) overlay (Xl, vj, f, fx): every reader of those is done
+    crba_fwd(P, Y, s, g);
+    if (a.H) DFX_FOR(e, DD) a.H[(long long)env * DD + e] = s[Y.A + e];
+    g.sync();
+    chol_inverse(P, Y, s, g);
+    solve_fwd(P, Y, s, g);
+    if (a.joint_qdd) DFX_FOR(i, D) a.joint_qdd[(long long)env * D + i] = s[Y.qdd + i];
+}
+
+// Adjoint, on the tape row and H^-1 block of a one-substep env-step from the same inputs (ta.tape_in: substeps = mm_freq = 1, fp32
+// rows, the external-wrench path; env_step_backward's loads): aq = aqd = 0, aqdd = g_qdd, the packed symmetrised cotangent of H
+// (Lm slot) = sym(g_H) -- g_H + g_H^T off the diagonal, as solve_adj keeps it -- instead of zero, then substep_adj<true, true>:
+// no integrator adjoint, g_tau joining the cotangent of tau after solve_adj.  Outputs as env_step_backward<true> writes them.
+template <class Grp>
+DFX_HD void dynamics_state_backward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const StepArgs& ta,
+                                    const DynamicsStateArgs& a) {
+    const int Q = P.Q, D = P.D, M = P.M, L = P.L, DD = D * D;
+    const RowFmt rf = row_fmt(P, Y, false);
+    const int xw = wrench_offset(Y, true);
+    DFX_FOR(i, D) s[Y.act + i] = a.act[(long long)env * D + i];
+    DFX_FOR(i, M) s[Y.musc + i] = a.musc[(long long)env * M + i];
+    DFX_FOR(i, L * 6) s[xw + i] = a.f_ext ? a.f_ext[(long long)env * L * 6 + i] : 0.0f;
+    DFX_FOR(i, L * 6) s[xw + L * 6 + i] = 0.0f;
+    DFX_FOR(i, D) s[Y.aact + i] = 0.0f;
+    DFX_FOR(i, M) s[Y.amusc + i] = 0.0f;
+    if (g.lane == 0) s[Y.cmask] = 0.0f;
+    if (M > 0) DFX_FOR(i, L * 13) s[Y.fxH + i] = 0.0f;
+    DFX_FOR(i, Q) s[Y.aq + i] = 0.0f;
+    DFX_FOR(i, D) s[Y.aqd + i] = 0.0f;
+    DFX_FOR(i, D) s[Y.aqdd + i] = a.g_qdd ? a.g_qdd[(long long)env * D + i] : 0.0f;
+    if constexpr (Grp::kBulkRows) {
+        g.rows_in(s + Y.q, ta.tape_in, 0, rf, s + Y.stage, s + (Y.A >= 0 ? Y.A : 0),
+                  Y.A >= 0 ? g.block_ptr(ta.tape_in + ta.hinv_base, 0, DD) : nullptr, DD);
+    } else {
+        g.row_in(s + Y.q, ta.tape_in, 0, ta.N, env, rf.n, rf.early, rf.tail, true);
+        if (Y.A >= 0) g.block_in(s + Y.A, ta.tape_in + ta.hinv_base, 0, ta.N, env, DD, false);
+    }
+    DFX_FOR(i, D) {                 // row i of the packed triangle: entries (i, i..D-1)
+        const SP row = s + Y.Lm + symD_idx(D, i, i);
+        if (a.g_H) {
+            const float* gH = a.g_H + (long long)env * DD;
+            row[0] = gH[i * D + i];
+            for (int j = i + 1; j < D; ++j) row[j - i] = gH[i * D + j] + gH[j * D + i];
+        } else {
+            for (int j = i; j < D; ++j) row[j - i] = 0.0f;
+        }
+    }
+    const HinvView hv = (Y.A >= 0) ? HinvView{nullptr, 0} : g.hinv_view(ta.tape_in + ta.hinv_base, 0, ta.N, env, DD);
+    if constexpr (!Grp::kBulkRows) g.row_in(s + Y.q, ta.tape_in, 0, ta.N, env, rf.n, rf.early, rf.tail, false);
+    g.copy_wait_first();
+    g.sync();
+    substep_adj<true, true>(P, Y, s, 0.0f, true, hv, rf, g, xw, a.g_tau ? a.g_tau + (long long)env * D : nullptr);
+    if (a.g_f_ext) DFX_FOR(i, L * 6) a.g_f_ext[(long long)env * L * 6 + i] = s[xw + L * 6 + i];
+    if (a.gq) DFX_FOR(i, Q) a.gq[(long long)env * Q + i] = s[Y.aq + i];
+    if (a.gqd) DFX_FOR(i, D) a.gqd[(long long)env * D + i] = s[Y.aqd + i];
+    if (a.gact) DFX_FOR(i, D) a.gact[(long long)env * D + i] = s[Y.aact + i];
+    if (a.gmusc) DFX_FOR(i, M) a.gmusc[(long long)env * M + i] = s[Y.amusc + i];
 }
 
 }  // namespace dfx

@@ -481,6 +481,99 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_contact_state_kernel(c
     else contact_state_forward(P, Y, s, g, env, ca);
 }
 
+// Dynamics state (include/dfx.h dfx_dynamics_state_forward; dfx_step.h dynamics_state_forward): the set-up of
+// dfx_tile_link_state_kernel line for line (keep the two in step) in the forward layout, with the external-wrench scratch, then the
+// first substep's dynamics up to the solve.
+template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_dynamics_state_kernel(const __grid_constant__ KernelArgs ka,
+                                                                               const __grid_constant__ DynamicsStateArgs da) {
+    constexpr int E = DFX_TILE_E;
+    extern __shared__ __align__(128) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += NW * 32) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += NW * 32) ipack[i] = ka.blob.ints[i];
+    int* cta_area = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    if (threadIdx.x < 4) cta_area[threadIdx.x] = 0;
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+    P.jmask = tile_joint_mask(SL, SD, SQ, SC, SM);
+    constexpr Layout Y = make_layout(SL, SD, SQ, SC, SM, MODE, false);
+
+    GroupTile<NW, E, PATH> g;
+    const int lane32 = threadIdx.x & 31;
+    g.lane = (threadIdx.x >> 5) * (32 / E) + lane32 / E;
+    g.e = lane32 % E;
+    g.tile = blockIdx.x;
+    g.ntiles = gridDim.x;
+    g.task_count = cta_area;
+    g.task_list = cta_area + 8;
+    g.mbar = nullptr;
+    g.par0 = g.par1 = 0u;
+    g.tile_base = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    int env = blockIdx.x * E + g.e;          // (lanes past the end redo the last environment, as in dfx_tile_kernel)
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const SP s{g.tile_base + g.e};
+    dynamics_state_forward(P, Y, s, g, env, da);
+}
+
+// Its adjoint (dfx_dynamics_state_backward; dfx_step.h dynamics_state_backward): the set-up and the fence / barrier sequence of
+// tile_recompute_body (keep the two in step), around a one-substep env-step forward that writes its tape row and H^-1 block into
+// the workspace ka.step.tape (fp32 rows), and the seeded adjoint that reads them back -- one launch.  The forward is the
+// external-wrench path with a NULL f_ext reading as zero: one forward in the kernel, with or without a wrench.
+template <int NW, int MINB, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_dynamics_backward_kernel(const __grid_constant__ KernelArgs ka,
+                                                                                  const __grid_constant__ DynamicsStateArgs da) {
+    constexpr int E = DFX_TILE_E;
+    extern __shared__ __align__(128) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += NW * 32) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += NW * 32) ipack[i] = ka.blob.ints[i];
+    int* cta_area = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    if (threadIdx.x < 4) cta_area[threadIdx.x] = 0;
+    unsigned long long* mbar = reinterpret_cast<unsigned long long*>(cta_area + 4);
+    if (threadIdx.x == 0) {
+        mbar_init(&mbar[0], 1);
+        mbar_init(&mbar[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+    P.jmask = tile_joint_mask(SL, SD, SQ, SC, SM);
+    constexpr Layout YF = make_layout(SL, SD, SQ, SC, SM, MODE, false);
+    constexpr Layout YB = make_layout(SL, SD, SQ, SC, SM, MODE, true);
+
+    GroupTile<NW, E, PATH> g;
+    const int lane32 = threadIdx.x & 31;
+    g.lane = (threadIdx.x >> 5) * (32 / E) + lane32 / E;
+    g.e = lane32 % E;
+    g.tile = blockIdx.x;
+    g.ntiles = gridDim.x;
+    g.task_count = cta_area;
+    g.task_list = cta_area + 8;
+    g.mbar = mbar;
+    g.par0 = g.par1 = 0u;
+    g.tile_base = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    int env = blockIdx.x * E + g.e;
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const SP s{g.tile_base + g.e};
+
+    env_step_forward<true, true>(P, YF, s, g, env, ka.step, ka.wrench);      // (ka.wrench.f_ext == da.f_ext; NULL reads as zero)
+    // (the sequence of tile_recompute_body: scratch writes fenced against the bulk loads, the tape's bulk stores written and
+    //  ordered before generic loads, both published by the barrier)
+    fence_async_smem();
+    if (threadIdx.x == 0) {
+        bulk_wait_all();
+        fence_async_global();
+    }
+    __syncthreads();
+    dynamics_state_backward(P, YB, s, g, env, ka.step, da);
+    g.finish();
+}
+
 // 128-byte aligned offsets so that the bulk copies of the tile stay 16-byte aligned
 static int tile_pack_floats(const KernelArgs& ka) {
     const int bytes = (((ka.blob.n_floats + 3) & ~3) + ((ka.blob.n_ints + 3) & ~3)) * 4;
@@ -511,12 +604,13 @@ static cudaError_t tile_launch(void (*kern)(P...), const Layout& Y, int per_env,
 }
 
 // what a tile entry point asks of the articulation's model entry (below): its layout mode, or a launch of one of its kernels
-enum class TileOp { mode, step, recompute, link_state, contact_state };
+enum class TileOp { mode, step, recompute, link_state, contact_state, dynamics_state };
 struct TileCall {
     TileOp op;
     bool backward, wrench;
     KernelArgs* ka;
-    const void* ra;         // the readout's kernel parameter: a LinkStateArgs (link_state) or a ContactStateArgs (contact_state)
+    const void* ra;         // the readout's kernel parameter: a LinkStateArgs (link_state), a ContactStateArgs (contact_state) or a
+                            // DynamicsStateArgs (dynamics_state)
     cudaStream_t stream;
 };
 
@@ -531,7 +625,8 @@ static int tile_model(const TileCall& c) {
     const int per_f = scratch_floats(YF, SL, false, c.wrench), per_b = scratch_floats(YB, SL, true, c.wrench);
     KernelArgs& ka = *c.ka;
     // (kernels referenced in the order of the step, its external-wrench twin, the recompute adjoint, the link state, the contact
-    //  state: nvcc emits the kernels in the order they are first referenced, and the code of some depends on that order)
+    //  state, the dynamics state: nvcc emits the kernels in the order they are first referenced, and the code of some depends on
+    //  that order)
     if (c.op == TileOp::step && !c.wrench)
         return c.backward ? tile_launch<NWB>(dfx_tile_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream)
                           : tile_launch<NWF>(dfx_tile_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream);
@@ -547,9 +642,15 @@ static int tile_model(const TileCall& c) {
             return c.backward ? tile_launch<NWB>(dfx_tile_link_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, la)
                               : tile_launch<NWF>(dfx_tile_link_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, la);
         }
-        const ContactStateArgs& ca = *static_cast<const ContactStateArgs*>(c.ra);
-        return c.backward ? tile_launch<NWB>(dfx_tile_contact_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, ca)
-                          : tile_launch<NWF>(dfx_tile_contact_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, ca);
+        if (c.op == TileOp::contact_state) {
+            const ContactStateArgs& ca = *static_cast<const ContactStateArgs*>(c.ra);
+            return c.backward ? tile_launch<NWB>(dfx_tile_contact_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, ca)
+                              : tile_launch<NWF>(dfx_tile_contact_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, ca);
+        }
+        // (the dynamics state: c.wrench is set, per_f / per_b include the wrench)
+        const DynamicsStateArgs& da = *static_cast<const DynamicsStateArgs*>(c.ra);
+        return c.backward ? tile_launch<NWB>(dfx_tile_dynamics_backward_kernel<NWB, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YB, dfx_max(per_f, per_b), ka, c.stream, da)
+                          : tile_launch<NWF>(dfx_tile_dynamics_state_kernel<NWF, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, da);
     }
     return -1;      // (the A/B variants are asked for the step only)
 }
@@ -647,12 +748,14 @@ static int tile_launch_recompute(void* kargs, int wrench, void* stream) {
     return tile_run(TileCall{TileOp::recompute, true, wrench != 0, static_cast<KernelArgs*>(kargs), nullptr, static_cast<cudaStream_t>(stream)}, false);
 }
 
-// a readout of (q, qd) -- op kReadoutLinkState: the link state (dfx_tile_link_state_kernel), kReadoutContactState: the contact state
-// (dfx_tile_contact_state_kernel) -- with the step kernels' warps and occupancy.  The flag-64 (A/B) variants have none: they run
-// these, which is valid because a readout has no tape layout to match.
+// a readout of the state -- op kReadoutLinkState: the link state (dfx_tile_link_state_kernel), kReadoutContactState: the contact
+// state (dfx_tile_contact_state_kernel), kReadoutDynamicsState: the dynamics state (dfx_tile_dynamics_state_kernel, and
+// dfx_tile_dynamics_backward_kernel with its own one-substep tape in the workspace) -- with the step kernels' warps and occupancy.
+// The flag-64 (A/B) variants have none: they run these, which is valid because a readout has no tape layout to match.
 static int tile_launch_readout(void* kargs, int op, const void* args, int backward, void* stream) {
-    const TileOp top = op == kReadoutContactState ? TileOp::contact_state : TileOp::link_state;
-    return tile_run(TileCall{top, backward != 0, false, static_cast<KernelArgs*>(kargs), args, static_cast<cudaStream_t>(stream)}, false);
+    const TileOp top = op == kReadoutContactState ? TileOp::contact_state : op == kReadoutDynamicsState ? TileOp::dynamics_state : TileOp::link_state;
+    return tile_run(TileCall{top, backward != 0, top == TileOp::dynamics_state, static_cast<KernelArgs*>(kargs), args,
+                             static_cast<cudaStream_t>(stream)}, false);
 }
 
 const DfxTileApi* DFX_TILE_FN(dfx_tile_api)(void) {

@@ -81,6 +81,7 @@ def check_link_input(engine, name, t, shapes):
 
 LINK_STATE_FIELDS = ("body_X_sc", "body_X_sm", "body_v_s")
 CONTACT_STATE_FIELDS = ("contact_f", "contact_height", "body_f_contact")
+DYNAMICS_STATE_FIELDS = ("joint_qdd", "joint_tau", "H")
 
 
 def wrench_struct(f_ext, g_f_ext=None):
@@ -405,6 +406,76 @@ class ArticulationEngine:
         _capi.check(code, "dfx_contact_state_backward")
         return gq, gqd
 
+    def _dynamics_state_inputs(self, q, qd, act, musc, f_ext):
+        if not hasattr(self.lib, "dfx_dynamics_state_forward"):
+            raise _capi.DfxError("%s has no dynamics-state entries (dfx_dynamics_state_*)" % _capi.LIB_PATH)
+        N, Q, D, M, L = self.N, self.Q, self.D, self.M, self.L
+        q = check_link_input(self, "q", q, ((N * Q,), (N, Q)))
+        qd = check_link_input(self, "qd", qd, ((N * D,), (N, D)))
+        act = check_link_input(self, "act", act, ((N * D,), (N, D)))
+        if act is None:
+            raise ValueError("act is required (zeros for no actuation)")
+        if M:
+            musc = check_link_input(self, "musc", musc, ((N * M,), (N, M)))
+            if musc is None:
+                raise ValueError("this model has muscles: musc is required")
+        else:
+            musc = None
+        f_ext = check_link_input(self, "f_ext", f_ext, ((N, L, 6), (N * L, 6), (N * L * 6,)))
+        return q, qd, act, musc, f_ext
+
+    def _dynamics_shapes(self):
+        N, D = self.N, self.D
+        return {"joint_qdd": ((N, D), (N * D,)), "joint_tau": ((N, D), (N * D,)), "H": ((N, D, D), (N * D, D), (N * D * D,))}
+
+    def dynamics_workspace(self):
+        """An uninitialised workspace for ``dynamics_state_backward``: one one-substep env-step's tape + its end state."""
+        n = int(self.lib.dfx_dynamics_workspace_floats(self.pack, self.N))
+        return torch.empty(n, dtype=torch.float32, device=self.device)
+
+    def dynamics_state(self, q, qd, act, musc=None, f_ext=None, want=DYNAMICS_STATE_FIELDS):
+        """(joint_qdd [N, D], joint_tau [N, D], H [N, D, D]) of the state (q, qd) under the actuation (act, musc) and the external
+        wrench f_ext (None: none) -- ``dfx_dynamics_state_forward``: what the first substep of an env-step from it computes before it
+        integrates.  joint_tau is the right-hand side of the solve (bias, contact, muscle and external forces, PD drive, act, limits),
+        not the actuator effort alone; H = J^T M J without the armature; joint_qdd = (H + diag(armature))^-1 joint_tau.  The fields
+        not in ``want`` are None (not computed).  q [N*Q] or [N, Q], qd and act [N*D] or [N, D], musc [N*M] or [N, M] (required
+        with muscles), f_ext [N, L, 6]; fp32 on the engine's device (ValueError otherwise)."""
+        return self._dynamics_state_checked(*self._dynamics_state_inputs(q, qd, act, musc, f_ext), want=want)
+
+    def _dynamics_state_checked(self, q, qd, act, musc, f_ext, want=DYNAMICS_STATE_FIELDS):
+        """``dynamics_state`` on inputs ``_dynamics_state_inputs`` has already checked and converted"""
+        shapes = self._dynamics_shapes()
+        out = tuple(torch.empty(shapes[name][0], dtype=torch.float32, device=self.device) if name in want else None
+                    for name in DYNAMICS_STATE_FIELDS)
+        with torch.cuda.device(self.device):
+            code = self.lib.dfx_dynamics_state_forward(self.pack, self.N, _ptr(q), _ptr(qd), _ptr(act), _ptr(musc), _ptr(f_ext),
+                                                       *(_ptr(o) for o in out), self._stream())
+        _capi.check(code, "dfx_dynamics_state_forward")
+        return out
+
+    def dynamics_state_backward(self, q, qd, act, musc, f_ext, g_qdd, g_tau, g_H, need=(True, True, True, True, True), workspace=None):
+        """Cotangents (gq [N*Q], gqd [N*D], gact [N*D], gmusc [N*M], g_f_ext [N, L, 6]) of the inputs from those of (joint_qdd,
+        joint_tau, H) (None: zero; g_H need not be symmetric) -- ``dfx_dynamics_state_backward``, which re-runs a one-substep
+        env-step into ``workspace`` (``dynamics_workspace()``; None: one from the caching allocator).  An output not in ``need``,
+        gmusc without muscles and g_f_ext without a wrench are None."""
+        q, qd, act, musc, f_ext = self._dynamics_state_inputs(q, qd, act, musc, f_ext)
+        shapes = self._dynamics_shapes()
+        g = [check_link_input(self, "g_" + name, t, shapes[name]) for name, t in zip(DYNAMICS_STATE_FIELDS, (g_qdd, g_tau, g_H))]
+        if workspace is None:
+            workspace = self.dynamics_workspace()
+        dev, N = self.device, self.N
+        gq = torch.empty(N * self.Q, dtype=torch.float32, device=dev) if need[0] else None
+        gqd = torch.empty(N * self.D, dtype=torch.float32, device=dev) if need[1] else None
+        gact = torch.empty(N * self.D, dtype=torch.float32, device=dev) if need[2] else None
+        gmusc = torch.empty(N * self.M, dtype=torch.float32, device=dev) if (need[3] and self.M) else None
+        g_f_ext = torch.empty((N, self.L, 6), dtype=torch.float32, device=dev) if (need[4] and f_ext is not None) else None
+        with torch.cuda.device(dev):
+            code = self.lib.dfx_dynamics_state_backward(self.pack, N, _ptr(q), _ptr(qd), _ptr(act), _ptr(musc), _ptr(f_ext),
+                                                        _ptr(workspace), *(_ptr(x) for x in g), _ptr(gq), _ptr(gqd), _ptr(gact),
+                                                        _ptr(gmusc), _ptr(g_f_ext), self._stream())
+        _capi.check(code, "dfx_dynamics_state_backward")
+        return gq, gqd, gact, gmusc, g_f_ext
+
 
 class MappedSimStepFunction(torch.autograd.Function):
     """(q, qd, raw policy output) -> (q', qd', used): the env-step with the action map folded into the simulation launch
@@ -527,6 +598,30 @@ class ContactStateFunction(torch.autograd.Function):
         g = [None if x is None else _f32c(x, dev) for x in (g_f, g_h, g_body)]
         gq, gqd = ctx.engine.contact_state_backward(q, qd, *g, need=tuple(ctx.needs_input_grad[1:3]))
         return None, None if gq is None else gq.view(ctx.shapes[0]), None if gqd is None else gqd.view(ctx.shapes[1])
+
+
+class DynamicsStateFunction(torch.autograd.Function):
+    """(q, qd, act, musc, f_ext) -> (joint_qdd [N, D], joint_tau [N, D], H [N, D, D]) (``ArticulationEngine.dynamics_state``).  Saves
+    only its inputs: the backward re-runs a one-substep env-step into a workspace it allocates, so it is the same in "tape" and
+    "recompute" adjoint mode.  musc and f_ext may be None."""
+
+    @staticmethod
+    def forward(ctx, engine, q, qd, act, musc, f_ext):
+        ins = engine._dynamics_state_inputs(q, qd, act, musc, f_ext)
+        out = engine._dynamics_state_checked(*ins)
+        ctx.engine = engine
+        ctx.shapes = tuple(None if t is None else t.shape for t in (q, qd, act, musc, f_ext))
+        ctx.set_materialize_grads(False)      # a missing cotangent is NULL for dfx_dynamics_state_backward, not a zero fill
+        ctx.save_for_backward(*ins)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_qdd, g_tau, g_H):
+        ins = ctx.saved_tensors
+        dev = ctx.engine.device
+        g = [None if x is None else _f32c(x, dev) for x in (g_qdd, g_tau, g_H)]
+        grads = ctx.engine.dynamics_state_backward(*ins, *g, need=tuple(ctx.needs_input_grad[1:6]))
+        return (None,) + tuple(None if x is None else x.view(s) for x, s in zip(grads, ctx.shapes))
 
 
 class SimStepFunction(torch.autograd.Function):

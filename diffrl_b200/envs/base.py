@@ -159,6 +159,25 @@ class DFlexEnv:
         from .. import contact_state
         return contact_state(self.model, self.state.joint_q, self.state.joint_qd)
 
+    def dynamics_state(self, actions):
+        """``diffrl_b200.dynamics_state`` of ``self.state`` under the actuation the env's action map makes of the policy output
+        ``actions`` [num_envs, num_actions] (``_action_map()`` through ``ActionMapFunction``: clipped, scaled, into joint_act or the
+        muscle activations, the other one zero, as the fused step forms them) and with the env's external wrench: what the next
+        ``step(actions)`` starts with.  ``DynamicsState(joint_qdd, joint_tau, H)``, [num_envs, D], [num_envs, D], [num_envs, D, D].
+        Differentiable: its gradient reaches ``actions``, the wrench and, through whichever step op produced ``self.state``, the
+        start state -- so a reward can penalise the torques or accelerations of the action about to be taken."""
+        from .. import dynamics_state
+        from ..env_ops import ActionMapFunction
+        if getattr(self, "_amap", None) is None:
+            self._amap = self._action_map()
+            self._tparams = self._transition_params()
+        width, offset, pre_scale, pre_bias, drive_scale, strength, is_muscle = self._amap
+        n = self.num_envs
+        _, drive = ActionMapFunction.apply(n, width, offset, pre_scale, pre_bias, drive_scale, strength, actions.view((n, self.num_actions)))
+        act = None if is_muscle else drive
+        musc = drive if is_muscle else None
+        return dynamics_state(self.model, self.state.joint_q, self.state.joint_qd, act, musc, self.external_wrench)
+
     def _attach_wrench(self, state):
         """The step reads the wrench from its input State (``body_f_ext``)."""
         if self.external_wrench is None:

@@ -410,6 +410,35 @@ int dfx_contact_state_backward(const dfx_pack_t* pack, int n, const float* q, co
                                const float* g_contact_f, const float* g_contact_height, const float* g_body_f_contact,
                                float* gq, float* gqd, void* stream);
 
+/* ---- dynamics state: joint accelerations, joint forces and mass matrix of (q, qd, act, musc, f_ext), differentiable -- what the
+ * first substep of an env-step from the state computes before it integrates (reference SemiImplicitIntegrator._simulate:
+ * eval_rigid_tau, eval_crba, eval_solve).  All fp32, env-major, in the Model's dof order:
+ *   joint_tau  [n*D]    State.joint_tau, the right-hand side of the solve: -S^T f of each joint's subtree (gravity, Coriolis and
+ *                       centrifugal terms, ground contacts, muscles and the external wrench), plus the PD drive to target, plus act,
+ *                       plus the joint-limit spring and damper; -f for a free joint.  NOT the actuator effort alone;
+ *   H          [n*D*D]  joint-space inertia J^T M J, row-major, symmetric, WITHOUT the armature;
+ *   joint_qdd  [n*D]    (H + diag(armature))^-1 joint_tau.
+ * H is always built from the given q (substep 0 of an env-step always refactorises).  act [n*D], musc [n*M] (required when M > 0),
+ * f_ext [n*L*6] in the DfxExternalWrench convention (NULL: no wrench).  The values are the derived dumps (DfxDerived joint_tau, H,
+ * joint_qdd) of a one-substep env-step from the same inputs, bit for bit.
+ *
+ * Backward: g_qdd, g_tau, g_H (NULL == 0; g_H need not be symmetric -- only g_H + g_H^T enters) -> gq [n*Q], gqd [n*D],
+ * gact [n*D], gmusc [n*M], g_f_ext [n*L*6] (overwritten; NULL: skip).  It re-runs a one-substep env-step from the inputs into
+ * `workspace` (device memory, dfx_dynamics_workspace_floats(pack, n) floats -- dfx_recompute_workspace_floats(pack, n, 1, 1) when
+ * the pack's tape is fp32 -- contents on entry ignored; its rows are fp32 whatever dfx_set_tape_dtype says) and runs the adjoint of
+ * that substep's dynamics on it, seeded with the cotangents and without the integrator: nothing is kept between the calls.
+ * Launches: forward one; backward one on the tile kernels (the forward into the workspace and the adjoint in the same CTA), two on
+ * the lane-group kernels (dfx_step_forward_ex into the workspace, then the adjoint).  Both run on the kernel family the step
+ * entries use (flag bit 6 of dfx_set_flags: the default tile kernels) and are bit-reproducible.  A NULL q, qd, act or workspace
+ * (backward), or a NULL musc when M > 0, is cudaErrorInvalidValue; with every output NULL there is no launch and 0 is returned.
+ * Stream-ordered, no host synchronisation. */
+long long dfx_dynamics_workspace_floats(const dfx_pack_t* pack, int n);
+int dfx_dynamics_state_forward(const dfx_pack_t* pack, int n, const float* q, const float* qd, const float* act, const float* musc,
+                               const float* f_ext, float* joint_qdd, float* joint_tau, float* H, void* stream);
+int dfx_dynamics_state_backward(const dfx_pack_t* pack, int n, const float* q, const float* qd, const float* act, const float* musc,
+                                const float* f_ext, float* workspace, const float* g_qdd, const float* g_tau, const float* g_H,
+                                float* gq, float* gqd, float* gact, float* gmusc, float* g_f_ext, void* stream);
+
 /* Launch configuration knob: lanes cooperating on one environment (8, 16 or 32; 0 = auto). */
 int dfx_set_group_size(int lanes);
 /* Tuning flags (default 9; for A/B timing and tests).  Lane-group kernels: bit 1 (2) = extra CTA-wide barriers between
