@@ -106,3 +106,28 @@ def dynamics_state(model, joint_q, joint_qd, joint_act=None, muscle_activation=N
 
 
 DynamicsState = collections.namedtuple("DynamicsState", ["joint_qdd", "joint_tau", "H"])
+
+
+def jacobian_state(model, joint_q, joint_qd):
+    """The link Jacobians and bias accelerations of the state (joint_q, joint_qd) of ``model``'s N environments, differentiable:
+    ``JacobianState(J, body_a_s)``, fp32, world axes (semantics in include/dfx.h, dfx_jacobian_state_forward) --
+
+    - ``J`` [N, L, 6, D]: the reference's model.J block per environment.  Column d of link i's 6 rows is the motion subspace
+      S_s[d] (spatial (w, v_o), the reference's joint_S_s) when dof d belongs to link i or one of its ancestors, exactly 0
+      otherwise; so ``body_v_s = J @ qd`` (``link_state``), and the columns of a free joint are the identity for every link;
+    - ``body_a_s`` [N, L, 6]: the reference State's body_a_s, J-dot qd: each link's spatial acceleration with qdd = 0, so the link
+      accelerations are ``J @ qdd + body_a_s`` (qdd from ``dynamics_state``).
+
+    Point Jacobians: for a point p fixed to link i (e.g. ``link_state(...).body_X_sm[:, i, :3]``, its centre of mass) with
+    (w, v_o) = body_v_s[:, i], dp/dt = (J_v - [p]x J_w) qd, J_w = J[:, i, :3], J_v = J[:, i, 3:]; its bias acceleration is
+    body_a_s.v + body_a_s.w x p + w x (v_o + w x p).
+
+    One kernel launch forward (include/dfx.h dfx_jacobian_state_forward) and one backward, which recomputes the kinematics from
+    (joint_q, joint_qd).  J depends on joint_q only; body_a_s on both.  joint_q [N*Q] or [N, Q], joint_qd [N*D] or [N, D], fp32 on
+    the model's device (ValueError otherwise); quaternions are used as given."""
+    from .dflex_api.sim import _engine_for
+    from .engine import JacobianStateFunction
+    return JacobianState(*JacobianStateFunction.apply(_engine_for(model), joint_q, joint_qd))
+
+
+JacobianState = collections.namedtuple("JacobianState", ["J", "body_a_s"])

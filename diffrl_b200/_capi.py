@@ -72,6 +72,9 @@ def lib():
     if hasattr(L, "dfx_link_state_forward"):    # link state of (q, qd) (include/dfx.h dfx_link_state_*)
         L.dfx_link_state_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, ctypes.c_void_p]
         L.dfx_link_state_backward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, _F, _F, ctypes.c_void_p]
+    if hasattr(L, "dfx_jacobian_state_forward"):    # Jacobian state of (q, qd) (include/dfx.h dfx_jacobian_state_*)
+        L.dfx_jacobian_state_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, ctypes.c_void_p]
+        L.dfx_jacobian_state_backward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, _F, ctypes.c_void_p]
     if hasattr(L, "dfx_contact_state_forward"):    # contact state of (q, qd) (include/dfx.h dfx_contact_state_*)
         L.dfx_contact_state_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, ctypes.c_void_p]
         L.dfx_contact_state_backward.argtypes = [ctypes.c_void_p, ctypes.c_int, _F, _F, _F, _F, _F, _F, _F, ctypes.c_void_p]

@@ -323,6 +323,45 @@ __global__ void __launch_bounds__(kMaxThreads) dfx_dynamics_state_kernel(const _
     else dynamics_state_forward(P, Y, s, g, env, da);
 }
 
+// Jacobian state (include/dfx.h dfx_jacobian_state_forward / _backward; dfx_step.h jacobian_state_*): the set-up of
+// dfx_link_state_kernel line for line (keep the two in step), then the kinematics of (q, qd) and the stores of J and body_a_s, or
+// their adjoint.
+template <int G, bool BACKWARD, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(kMaxThreads) dfx_jacobian_state_kernel(const __grid_constant__ KernelArgs ka,
+                                                                       const __grid_constant__ JacobianStateArgs ja) {
+    extern __shared__ __align__(16) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += blockDim.x) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += blockDim.x) ipack[i] = ka.blob.ints[i];
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    Layout Y = ka.layout;
+    if constexpr (SL > 0) {
+        P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+        constexpr Layout kY = make_layout(SL, SD, SQ, SC, SM);
+        Y = kY;
+    }
+    const int kEnvsPerCta = blockDim.x / G;
+    const int local = threadIdx.x / G;
+    int env = blockIdx.x * kEnvsPerCta + local;      // (groups past the end redo the last environment, as in step_kernel_body)
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const int lane_in_warp = threadIdx.x & 31;
+    GroupCuda<G> g;
+    g.lane = threadIdx.x % G;
+    g.psync = (ka.step.flags & 2) != 0;
+    g.mask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << ((lane_in_warp / G) * G));
+    float* s = smem + ka.pack_smem_floats + ka.cta_area_floats + (size_t)local * ka.scratch_stride;
+    g.scratch0 = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    g.task_count = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    g.task_list = g.task_count + 4;
+    g.stride = ka.scratch_stride;
+    g.envs_shift = 31 - __clz(kEnvsPerCta > 0 ? kEnvsPerCta : 1);
+    g.cta_mode = (ka.step.flags & 8) != 0;
+    if (BACKWARD) jacobian_state_backward(P, Y, s, g, env, ja);
+    else jacobian_state_forward(P, Y, s, g, env, ja);
+}
+
 }  // namespace dfx
 
 // =====================================================================================
@@ -531,11 +570,11 @@ static int counted(int e) {
 }
 
 // the lane-group kernel families
-enum GroupFamily { kStep, kStepWrench, kLinkState, kContactState, kDynamicsState };
+enum GroupFamily { kStep, kStepWrench, kLinkState, kContactState, kDynamicsState, kJacobianState };
 
 // one lane-group launch: the family's kernel of group width G, size-specialised (SL..SM > 0) or generic, with plan_launch's
-// geometry; ra: the readout's kernel parameter (a LinkStateArgs, ContactStateArgs or DynamicsStateArgs), NULL for the step
-// families.  The external-wrench step and the dynamics state keep the wrench past the layout's end.
+// geometry; ra: the readout's kernel parameter (a LinkStateArgs, ContactStateArgs, DynamicsStateArgs or JacobianStateArgs), NULL
+// for the step families.  The external-wrench step and the dynamics state keep the wrench past the layout's end.
 template <GroupFamily F, int G, bool BWD, int SL, int SD, int SQ, int SC, int SM>
 static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const void* ra, cudaStream_t stream) {
     ka.layout = BWD ? p->host.layout_bwd : p->host.layout;
@@ -559,6 +598,8 @@ static cudaError_t launch_impl(const dfx_pack* p, KernelArgs& ka, const void* ra
         return go(dfx_contact_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *static_cast<const ContactStateArgs*>(ra));
     } else if constexpr (F == kDynamicsState) {
         return go(dfx_dynamics_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *static_cast<const DynamicsStateArgs*>(ra));
+    } else if constexpr (F == kJacobianState) {
+        return go(dfx_jacobian_state_kernel<G, BWD, SL, SD, SQ, SC, SM>, *static_cast<const JacobianStateArgs*>(ra));
     } else {
         // (the step kernel is referenced before its external-wrench twin, in every instantiation: nvcc emits the kernels in the
         //  order they are first referenced, and the code of some depends on that order)
@@ -749,6 +790,16 @@ static int run_dynamics_state(const dfx_pack_t* p, int n, const DynamicsStateArg
         if (e != 0) return e;
     }
     return run_group<kDynamicsState>(p, ka, backward, &da, (cudaStream_t)stream);
+}
+
+// ---- Jacobian state (include/dfx.h dfx_jacobian_state_*): on the kernels run_link_state picks
+static int run_jacobian_state(const dfx_pack_t* p, int n, const JacobianStateArgs& ja, bool backward, void* stream) {
+    StepArgs a{};
+    a.N = n;
+    a.flags = g_flags;
+    KernelArgs ka = kernel_args(p, a, nullptr);
+    if (p->tile) return counted(tile_api(p->tile)->launch_readout(&ka, kReadoutJacobianState, &ja, backward, stream));
+    return run_group<kJacobianState>(p, ka, backward, &ja, (cudaStream_t)stream);
 }
 
 extern "C" {
@@ -1065,6 +1116,25 @@ int dfx_dynamics_state_backward(const dfx_pack_t* p, int n, const float* q, cons
     da.g_qdd = g_qdd; da.g_tau = g_tau; da.g_H = g_H;
     da.gq = gq; da.gqd = gqd; da.gact = gact; da.gmusc = gmusc; da.g_f_ext = g_f_ext;
     return run_dynamics_state(p, n, da, workspace, true, stream);
+}
+
+int dfx_jacobian_state_forward(const dfx_pack_t* p, int n, const float* q, const float* qd, float* J, float* body_a_s, void* stream) {
+    if (!p || n <= 0 || !q || !qd) return (int)cudaErrorInvalidValue;
+    if (!J && !body_a_s) return 0;
+    JacobianStateArgs ja;
+    memset(&ja, 0, sizeof ja);
+    ja.q = q; ja.qd = qd; ja.J = J; ja.a_s = body_a_s;
+    return run_jacobian_state(p, n, ja, false, stream);
+}
+
+int dfx_jacobian_state_backward(const dfx_pack_t* p, int n, const float* q, const float* qd, const float* g_J, const float* g_a_s,
+                                float* gq, float* gqd, void* stream) {
+    if (!p || n <= 0 || !q || !qd) return (int)cudaErrorInvalidValue;
+    if (!gq && !gqd) return 0;
+    JacobianStateArgs ja;
+    memset(&ja, 0, sizeof ja);
+    ja.q = q; ja.qd = qd; ja.g_J = g_J; ja.g_a_s = g_a_s; ja.gq = gq; ja.gqd = gqd;
+    return run_jacobian_state(p, n, ja, true, stream);
 }
 
 }  // extern "C"

@@ -81,11 +81,12 @@ struct DfxTileApi {
     size_t (*smem)(const void* kernel_args, int backward);   // dynamic shared memory (bytes); backward: bit 0 adjoint, bit 1 wrench
     int (*launch)(void* kernel_args, int backward, int wrench, void* stream);   // wrench != 0: the external-wrench kernels
     int (*launch_recompute)(void* kernel_args, int wrench, void* stream);       // forward into the workspace + adjoint, one launch
-    // a readout of the state -- op: DfxReadout; args: its LinkStateArgs, ContactStateArgs or DynamicsStateArgs.  The dynamics
-    // state's backward is one launch: the one-substep forward into the workspace kernel_args->step.tape, then the seeded adjoint
+    // a readout of the state -- op: DfxReadout; args: its LinkStateArgs, ContactStateArgs, DynamicsStateArgs or JacobianStateArgs.
+    // The dynamics state's backward is one launch: the one-substep forward into the workspace kernel_args->step.tape, then the
+    // seeded adjoint
     int (*launch_readout)(void* kernel_args, int op, const void* args, int backward, void* stream);
 };
-enum DfxReadout { kReadoutLinkState = 0, kReadoutContactState = 1, kReadoutDynamicsState = 2 };
+enum DfxReadout { kReadoutLinkState = 0, kReadoutContactState = 1, kReadoutDynamicsState = 2, kReadoutJacobianState = 3 };
 const DfxTileApi* dfx_tile_api_e8(void);
 const DfxTileApi* dfx_tile_api_e16(void);
 const DfxTileApi* dfx_tile_api_e32(void);

@@ -529,4 +529,70 @@ DFX_HD void dynamics_state_backward(const Pack& P, const Layout& Y, SP s, const 
     if (a.gmusc) DFX_FOR(i, M) a.gmusc[(long long)env * M + i] = s[Y.amusc + i];
 }
 
+// ---- Jacobian state of (q, qd) (include/dfx.h dfx_jacobian_state_forward / _backward): the link Jacobians J [L, 6, D] -- column d
+// of link i's block is S[d] when dof d moves link i (a dof of i or of an ancestor: the pack's anc_dofs list of i), 0 otherwise -- and
+// the bias accelerations a (reference State body_a_s, J-dot qd), both from the kinematics link_state_kinematics leaves in the scratch.
+struct JacobianStateArgs {
+    const float* q; const float* qd;
+    float* J; float* a_s;                           // forward outputs [N, L, 6, D], [N, L, 6] (NULL: skip)
+    const float* g_J; const float* g_a_s;           // backward: their cotangents (NULL == 0)
+    float* gq; float* gqd;                          // backward outputs [N, Q], [N, D] (NULL: skip)
+};
+
+// element k = (i * 6 + r) * D + d of one environment's J: S[d][r] when d is in link i's ancestor-or-self dof list (ascending), else 0
+DFX_HD float jacobian_entry(const Pack& P, const Layout& Y, SP s, int k) {
+    const int D = P.D, d = k % D, ir = k / D, i = ir / 6, r = ir - i * 6;
+    for (int j = P.anc_start[i]; j < P.anc_start[i + 1]; ++j) {
+        const int a = P.anc_dofs[j];
+        if (a >= d) return a == d ? s[Y.S + d * 6 + r] : 0.0f;
+    }
+    return 0.0f;
+}
+
+// every element of J is written (zeros included), one environment per item group
+template <class Grp>
+DFX_HD void jacobian_state_forward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const JacobianStateArgs& a) {
+    const int L = P.L, LD6 = L * 6 * P.D;
+    LinkStateArgs la{};
+    la.q = a.q; la.qd = a.qd;
+    link_state_kinematics(P, Y, s, g, env, la);
+    if (a.J) DFX_FOR(k, LD6) a.J[(long long)env * LD6 + k] = jacobian_entry(P, Y, s, k);
+    if (a.a_s) DFX_FOR(i, L * 6) a.a_s[(long long)env * L * 6 + i] = s[Y.a + i];
+}
+
+// adjoint: the kinematics recomputed from (q, qd); aS[d][r] = the sum of g_J[l][r][d] over the links l that dof d moves (the subtree
+// of its link, sub_links in list order; one item per link over its dofs and rows -- no atomics, so the sums are bit-reproducible),
+// aa = g_a_s, the other cotangents zero; then A1 for every link and the rest of the kinematics adjoint, as link_state_backward
+template <class Grp>
+DFX_HD void jacobian_state_backward(const Pack& P, const Layout& Y, SP s, const Grp& g, int env, const JacobianStateArgs& a) {
+    const int L = P.L, Q = P.Q, D = P.D, LD6 = L * 6 * D;
+    LinkStateArgs la{};
+    la.q = a.q; la.qd = a.qd;
+    link_state_kinematics(P, Y, s, g, env, la);
+    DFX_FOR(i, L * 7) s[Y.aXsc + i] = 0.0f;
+    DFX_FOR(i, L * 7) s[Y.aXsm + i] = 0.0f;
+    DFX_FOR(i, L * 6) s[Y.av + i] = 0.0f;
+    DFX_FOR(i, L * 6) s[Y.aa + i] = a.g_a_s ? a.g_a_s[(long long)env * L * 6 + i] : 0.0f;
+    DFX_FOR(i, L) {          // (one item per link, over its dofs and rows)
+        for (int d = P.qd_start[i]; d < P.qd_start[i + 1]; ++d) {
+            for (int r = 0; r < 6; ++r) {
+                float acc = 0.0f;
+                if (a.g_J)
+                    for (int k = P.sub_start[i]; k < P.sub_start[i + 1]; ++k)
+                        acc += a.g_J[(long long)env * LD6 + (P.sub_links[k] * 6 + r) * D + d];
+                s[Y.aS + d * 6 + r] = acc;
+            }
+        }
+    }
+    DFX_FOR(i, Q) s[Y.aq + i] = 0.0f;
+    DFX_FOR(i, D) s[Y.aqd + i] = 0.0f;
+    g.sync();
+    DFX_FOR(i, L) kin_adj_local(P, Y, s, i);
+    g.sync();
+    kin_adj(P, Y, s, g);
+    g.sync();
+    if (a.gq) DFX_FOR(i, Q) a.gq[(long long)env * Q + i] = s[Y.aq + i];
+    if (a.gqd) DFX_FOR(i, D) a.gqd[(long long)env * D + i] = s[Y.aqd + i];
+}
+
 }  // namespace dfx

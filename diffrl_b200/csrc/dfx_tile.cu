@@ -574,6 +574,45 @@ __global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_dynamics_backward_kern
     g.finish();
 }
 
+// Jacobian state (include/dfx.h dfx_jacobian_state_forward / _backward; dfx_step.h jacobian_state_*): the set-up of
+// dfx_tile_link_state_kernel line for line (keep the two in step), then the kinematics of (q, qd) and the stores of J and body_a_s, or
+// their adjoint.  J is stored per environment, as the link state's outputs (DESIGN.md: a CTA-wide coalesced store of the tile's J was
+// slower on the humanoids' E = 8 and 16 tiles).
+template <int NW, int MINB, bool BACKWARD, bool PATH, int MODE, int SL, int SD, int SQ, int SC, int SM>
+__global__ void __launch_bounds__(NW * 32, MINB) dfx_tile_jacobian_state_kernel(const __grid_constant__ KernelArgs ka,
+                                                                               const __grid_constant__ JacobianStateArgs ja) {
+    constexpr int E = DFX_TILE_E;
+    extern __shared__ __align__(128) float smem[];
+    float* fpack = smem;
+    int* ipack = reinterpret_cast<int*>(smem + ((ka.blob.n_floats + 3) & ~3));
+    for (int i = threadIdx.x; i < ka.blob.n_floats; i += NW * 32) fpack[i] = ka.blob.floats[i];
+    for (int i = threadIdx.x; i < ka.blob.n_ints; i += NW * 32) ipack[i] = ka.blob.ints[i];
+    int* cta_area = reinterpret_cast<int*>(smem + ka.pack_smem_floats);
+    if (threadIdx.x < 4) cta_area[threadIdx.x] = 0;
+    __syncthreads();
+    Pack P = bind_pack(ka.header, ka.blob, ipack, fpack);
+    P.L = SL; P.D = SD; P.Q = SQ; P.C = SC; P.M = SM;
+    P.jmask = tile_joint_mask(SL, SD, SQ, SC, SM);
+    constexpr Layout Y = make_layout(SL, SD, SQ, SC, SM, MODE, BACKWARD);
+
+    GroupTile<NW, E, PATH> g;
+    const int lane32 = threadIdx.x & 31;
+    g.lane = (threadIdx.x >> 5) * (32 / E) + lane32 / E;
+    g.e = lane32 % E;
+    g.tile = blockIdx.x;
+    g.ntiles = gridDim.x;
+    g.task_count = cta_area;
+    g.task_list = cta_area + 8;
+    g.mbar = nullptr;
+    g.par0 = g.par1 = 0u;
+    g.tile_base = smem + ka.pack_smem_floats + ka.cta_area_floats;
+    int env = blockIdx.x * E + g.e;          // (lanes past the end redo the last environment, as in dfx_tile_kernel)
+    if (env >= ka.step.N) env = ka.step.N - 1;
+    const SP s{g.tile_base + g.e};
+    if (BACKWARD) jacobian_state_backward(P, Y, s, g, env, ja);
+    else jacobian_state_forward(P, Y, s, g, env, ja);
+}
+
 // 128-byte aligned offsets so that the bulk copies of the tile stay 16-byte aligned
 static int tile_pack_floats(const KernelArgs& ka) {
     const int bytes = (((ka.blob.n_floats + 3) & ~3) + ((ka.blob.n_ints + 3) & ~3)) * 4;
@@ -604,13 +643,13 @@ static cudaError_t tile_launch(void (*kern)(P...), const Layout& Y, int per_env,
 }
 
 // what a tile entry point asks of the articulation's model entry (below): its layout mode, or a launch of one of its kernels
-enum class TileOp { mode, step, recompute, link_state, contact_state, dynamics_state };
+enum class TileOp { mode, step, recompute, link_state, contact_state, dynamics_state, jacobian_state };
 struct TileCall {
     TileOp op;
     bool backward, wrench;
     KernelArgs* ka;
-    const void* ra;         // the readout's kernel parameter: a LinkStateArgs (link_state), a ContactStateArgs (contact_state) or a
-                            // DynamicsStateArgs (dynamics_state)
+    const void* ra;         // the readout's kernel parameter: a LinkStateArgs (link_state), a ContactStateArgs (contact_state), a
+                            // DynamicsStateArgs (dynamics_state) or a JacobianStateArgs (jacobian_state)
     cudaStream_t stream;
 };
 
@@ -625,8 +664,8 @@ static int tile_model(const TileCall& c) {
     const int per_f = scratch_floats(YF, SL, false, c.wrench), per_b = scratch_floats(YB, SL, true, c.wrench);
     KernelArgs& ka = *c.ka;
     // (kernels referenced in the order of the step, its external-wrench twin, the recompute adjoint, the link state, the contact
-    //  state, the dynamics state: nvcc emits the kernels in the order they are first referenced, and the code of some depends on
-    //  that order)
+    //  state, the dynamics state, the Jacobian state: nvcc emits the kernels in the order they are first referenced, and the code of
+    //  some depends on that order)
     if (c.op == TileOp::step && !c.wrench)
         return c.backward ? tile_launch<NWB>(dfx_tile_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream)
                           : tile_launch<NWF>(dfx_tile_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream);
@@ -647,10 +686,14 @@ static int tile_model(const TileCall& c) {
             return c.backward ? tile_launch<NWB>(dfx_tile_contact_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, ca)
                               : tile_launch<NWF>(dfx_tile_contact_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, ca);
         }
-        // (the dynamics state: c.wrench is set, per_f / per_b include the wrench)
-        const DynamicsStateArgs& da = *static_cast<const DynamicsStateArgs*>(c.ra);
-        return c.backward ? tile_launch<NWB>(dfx_tile_dynamics_backward_kernel<NWB, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YB, dfx_max(per_f, per_b), ka, c.stream, da)
-                          : tile_launch<NWF>(dfx_tile_dynamics_state_kernel<NWF, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, da);
+        if (c.op == TileOp::dynamics_state) {      // (c.wrench is set, per_f / per_b include the wrench)
+            const DynamicsStateArgs& da = *static_cast<const DynamicsStateArgs*>(c.ra);
+            return c.backward ? tile_launch<NWB>(dfx_tile_dynamics_backward_kernel<NWB, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YB, dfx_max(per_f, per_b), ka, c.stream, da)
+                              : tile_launch<NWF>(dfx_tile_dynamics_state_kernel<NWF, MINB, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, da);
+        }
+        const JacobianStateArgs& ja = *static_cast<const JacobianStateArgs*>(c.ra);
+        return c.backward ? tile_launch<NWB>(dfx_tile_jacobian_state_kernel<NWB, MINB, true, PATH, LM, SL, SD, SQ, SC, SM>, YB, per_b, ka, c.stream, ja)
+                          : tile_launch<NWF>(dfx_tile_jacobian_state_kernel<NWF, MINB, false, PATH, LM, SL, SD, SQ, SC, SM>, YF, per_f, ka, c.stream, ja);
     }
     return -1;      // (the A/B variants are asked for the step only)
 }
@@ -750,10 +793,12 @@ static int tile_launch_recompute(void* kargs, int wrench, void* stream) {
 
 // a readout of the state -- op kReadoutLinkState: the link state (dfx_tile_link_state_kernel), kReadoutContactState: the contact
 // state (dfx_tile_contact_state_kernel), kReadoutDynamicsState: the dynamics state (dfx_tile_dynamics_state_kernel, and
-// dfx_tile_dynamics_backward_kernel with its own one-substep tape in the workspace) -- with the step kernels' warps and occupancy.
+// dfx_tile_dynamics_backward_kernel with its own one-substep tape in the workspace), kReadoutJacobianState: the Jacobian state
+// (dfx_tile_jacobian_state_kernel) -- with the step kernels' warps and occupancy.
 // The flag-64 (A/B) variants have none: they run these, which is valid because a readout has no tape layout to match.
 static int tile_launch_readout(void* kargs, int op, const void* args, int backward, void* stream) {
-    const TileOp top = op == kReadoutContactState ? TileOp::contact_state : op == kReadoutDynamicsState ? TileOp::dynamics_state : TileOp::link_state;
+    const TileOp top = op == kReadoutContactState ? TileOp::contact_state : op == kReadoutDynamicsState ? TileOp::dynamics_state
+                     : op == kReadoutJacobianState ? TileOp::jacobian_state : TileOp::link_state;
     return tile_run(TileCall{top, backward != 0, top == TileOp::dynamics_state, static_cast<KernelArgs*>(kargs), args,
                              static_cast<cudaStream_t>(stream)}, false);
 }

@@ -82,6 +82,7 @@ def check_link_input(engine, name, t, shapes):
 LINK_STATE_FIELDS = ("body_X_sc", "body_X_sm", "body_v_s")
 CONTACT_STATE_FIELDS = ("contact_f", "contact_height", "body_f_contact")
 DYNAMICS_STATE_FIELDS = ("joint_qdd", "joint_tau", "H")
+JACOBIAN_STATE_FIELDS = ("J", "body_a_s")
 
 
 def wrench_struct(f_ext, g_f_ext=None):
@@ -406,6 +407,44 @@ class ArticulationEngine:
         _capi.check(code, "dfx_contact_state_backward")
         return gq, gqd
 
+    def _jacobian_state_inputs(self, q, qd):
+        if not hasattr(self.lib, "dfx_jacobian_state_forward"):
+            raise _capi.DfxError("%s has no Jacobian-state entries (dfx_jacobian_state_*)" % _capi.LIB_PATH)
+        q = check_link_input(self, "q", q, ((self.N * self.Q,), (self.N, self.Q)))
+        qd = check_link_input(self, "qd", qd, ((self.N * self.D,), (self.N, self.D)))
+        return q, qd
+
+    def jacobian_state(self, q, qd, want=JACOBIAN_STATE_FIELDS):
+        """(J [N, L, 6, D], body_a_s [N, L, 6]) of the state (q, qd) -- ``dfx_jacobian_state_forward`` (semantics in include/dfx.h):
+        the link Jacobians, column d of link i's block the motion subspace S_s[d] (spatial (w, v_o), world axes) when dof d moves
+        link i and exactly 0 otherwise, so body_v_s = J @ qd; and the bias accelerations J-dot qd, so the link accelerations are
+        J @ qdd + body_a_s.  The fields not in ``want`` are None (not computed).  q [N*Q] or [N, Q], qd [N*D] or [N, D], fp32 on the
+        engine's device (ValueError otherwise); quaternions are used as given."""
+        q, qd = self._jacobian_state_inputs(q, qd)
+        N, L, D = self.N, self.L, self.D
+        out = (torch.empty((N, L, 6, D), dtype=torch.float32, device=self.device) if "J" in want else None,
+               torch.empty((N, L, 6), dtype=torch.float32, device=self.device) if "body_a_s" in want else None)
+        with torch.cuda.device(self.device):
+            code = self.lib.dfx_jacobian_state_forward(self.pack, N, _ptr(q), _ptr(qd), *(_ptr(o) for o in out), self._stream())
+        _capi.check(code, "dfx_jacobian_state_forward")
+        return out
+
+    def jacobian_state_backward(self, q, qd, g_J, g_a_s, need=(True, True)):
+        """Cotangents (gq [N*Q], gqd [N*D]) of the state from those of (J, body_a_s) (None: zero; g_J as [N, L, 6, D], [N, 6L, D]
+        or flat) -- ``dfx_jacobian_state_backward``, which recomputes the kinematics of (q, qd).  J depends on q only.  An output
+        not in ``need`` is None."""
+        q, qd = self._jacobian_state_inputs(q, qd)
+        N, L, D = self.N, self.L, self.D
+        g_J = check_link_input(self, "g_J", g_J, ((N, L, 6, D), (N, 6 * L, D), (N * L * 6 * D,)))
+        g_a_s = check_link_input(self, "g_body_a_s", g_a_s, ((N, L, 6), (N * L, 6), (N * L * 6,)))
+        gq = torch.empty(N * self.Q, dtype=torch.float32, device=self.device) if need[0] else None
+        gqd = torch.empty(N * self.D, dtype=torch.float32, device=self.device) if need[1] else None
+        with torch.cuda.device(self.device):
+            code = self.lib.dfx_jacobian_state_backward(self.pack, N, _ptr(q), _ptr(qd), _ptr(g_J), _ptr(g_a_s), _ptr(gq), _ptr(gqd),
+                                                        self._stream())
+        _capi.check(code, "dfx_jacobian_state_backward")
+        return gq, gqd
+
     def _dynamics_state_inputs(self, q, qd, act, musc, f_ext):
         if not hasattr(self.lib, "dfx_dynamics_state_forward"):
             raise _capi.DfxError("%s has no dynamics-state entries (dfx_dynamics_state_*)" % _capi.LIB_PATH)
@@ -622,6 +661,29 @@ class DynamicsStateFunction(torch.autograd.Function):
         g = [None if x is None else _f32c(x, dev) for x in (g_qdd, g_tau, g_H)]
         grads = ctx.engine.dynamics_state_backward(*ins, *g, need=tuple(ctx.needs_input_grad[1:6]))
         return (None,) + tuple(None if x is None else x.view(s) for x, s in zip(grads, ctx.shapes))
+
+
+class JacobianStateFunction(torch.autograd.Function):
+    """(q, qd) -> (J [N, L, 6, D], body_a_s [N, L, 6]): the link Jacobians and bias accelerations
+    (``ArticulationEngine.jacobian_state``).  Saves only (q, qd): the backward recomputes the kinematics, so it is the same in
+    "tape" and "recompute" adjoint mode."""
+
+    @staticmethod
+    def forward(ctx, engine, q, qd):
+        qc, qdc = engine._jacobian_state_inputs(q, qd)
+        out = engine.jacobian_state(qc, qdc)
+        ctx.engine, ctx.shapes = engine, (q.shape, qd.shape)
+        ctx.set_materialize_grads(False)      # a missing cotangent is NULL for dfx_jacobian_state_backward, not a zero fill
+        ctx.save_for_backward(qc, qdc)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_J, g_a_s):
+        q, qd = ctx.saved_tensors
+        dev = ctx.engine.device
+        g = [None if x is None else _f32c(x, dev) for x in (g_J, g_a_s)]
+        gq, gqd = ctx.engine.jacobian_state_backward(q, qd, *g, need=tuple(ctx.needs_input_grad[1:3]))
+        return None, None if gq is None else gq.view(ctx.shapes[0]), None if gqd is None else gqd.view(ctx.shapes[1])
 
 
 class SimStepFunction(torch.autograd.Function):

@@ -159,6 +159,13 @@ class DFlexEnv:
         from .. import contact_state
         return contact_state(self.model, self.state.joint_q, self.state.joint_qd)
 
+    def jacobian_state(self):
+        """``diffrl_b200.jacobian_state`` of ``self.state``, the state the next step starts from: ``JacobianState(J, body_a_s)``,
+        [num_envs, L, 6, D], [num_envs, L, 6].  Differentiable: its gradient reaches the actions and the start state through
+        whichever step op produced ``self.state``."""
+        from .. import jacobian_state
+        return jacobian_state(self.model, self.state.joint_q, self.state.joint_qd)
+
     def dynamics_state(self, actions):
         """``diffrl_b200.dynamics_state`` of ``self.state`` under the actuation the env's action map makes of the policy output
         ``actions`` [num_envs, num_actions] (``_action_map()`` through ``ActionMapFunction``: clipped, scaled, into joint_act or the

@@ -439,6 +439,32 @@ int dfx_dynamics_state_backward(const dfx_pack_t* pack, int n, const float* q, c
                                 const float* f_ext, float* workspace, const float* g_qdd, const float* g_tau, const float* g_H,
                                 float* gq, float* gqd, float* gact, float* gmusc, float* g_f_ext, void* stream);
 
+/* ---- Jacobian state: the link Jacobians and bias accelerations of (q, qd), differentiable.  At a state of n environments (fp32,
+ * environment-major):
+ *   J        [n*L*6*D]  the reference's per-articulation model.J block (spatial_jacobian, spatial.h:691-738): row 6 i + r, column d
+ *                       at (6 i + r) * D + d.  Column d of link i's rows is the motion subspace S_s[d] of dof d (the reference's
+ *                       joint_S_s: a spatial (w, v_o) twist in world axes) when dof d belongs to link i or to one of its ancestors,
+ *                       and exactly 0 otherwise.  So body_v_s[i] = J[i] qd (dfx_link_state_forward), and the columns of a free
+ *                       joint are the identity for every link of its tree.  Quaternions in q are used as given, as the link state.
+ *   body_a_s [n*L*6]    the reference State's body_a_s (eval_rigid_fk / eval_rigid_id, sim.py:1763): each link's spatial
+ *                       acceleration with q'' = 0, i.e. J-dot qd, in the same (w, v_o) convention.  The full link acceleration is
+ *                       J q'' + body_a_s, with q'' from dfx_dynamics_state_forward.
+ * Point Jacobians.  A point p fixed to link i (e.g. its centre of mass, X_sm.p of the link state) moves with v_o + w x p, where
+ * (w, v_o) = body_v_s[i].  With J_w the rows 0-2 and J_v the rows 3-5 of link i's block:
+ *   dp/dt   = (J_v - [p]x J_w) qd,
+ *   d2p/dt2 = (J_v - [p]x J_w) q'' + b,   b = body_a_s[i].v + body_a_s[i].w x p + w x (v_o + w x p),
+ * b being the point's bias acceleration: the spatial acceleration a = (a_w, a_v) gives a point the acceleration
+ * a_v + a_w x p + w x dp/dt, and the last term is the w x (w x p)-type term of the spatial convention.
+ * Gradients: J depends on q only (its cotangent reaches gq); body_a_s on (q, qd).  The backward recomputes the kinematics from
+ * (q, qd) and keeps nothing between the calls.  Both run on the kernel family the step entries use, in the step's scratch layouts (an
+ * articulation the step fits, these fit), one launch each, and are bit-reproducible.  A NULL q or qd is cudaErrorInvalidValue; a
+ * NULL output is skipped, a NULL cotangent is zero; with every output NULL there is no launch and 0 is returned.  Stream-ordered, no
+ * host synchronisation. */
+int dfx_jacobian_state_forward(const dfx_pack_t* pack, int n, const float* q, const float* qd, float* J, float* body_a_s, void* stream);
+/* cotangents g_J [n*L*6*D], g_a_s [n*L*6] (NULL == 0) -> gq [n*Q], gqd [n*D] (overwritten; NULL: skip) */
+int dfx_jacobian_state_backward(const dfx_pack_t* pack, int n, const float* q, const float* qd, const float* g_J, const float* g_a_s,
+                                float* gq, float* gqd, void* stream);
+
 /* Launch configuration knob: lanes cooperating on one environment (8, 16 or 32; 0 = auto). */
 int dfx_set_group_size(int lanes);
 /* Tuning flags (default 9; for A/B timing and tests).  Lane-group kernels: bit 1 (2) = extra CTA-wide barriers between
